@@ -233,7 +233,7 @@ __device__ int warp_backtrack_step(const RowTables &rt, const DpState &d, const 
     const int npre = rc.base_npre >> 8;
     const int s = smat8[8 * (rc.base_npre & 0xff) + q[j - 1]];
     int hij = inf; unsigned cij = (unsigned)E_NEG16 | (unsigned)E_NEG16 << 16;
-    if (j >= ri.beg && j <= ri.end) { const int64_t o = plane_index(ri.beg, ri.end, 0, j); hij = __ldcg(rowi + o); cij = (unsigned)__ldcg(rowi + o + CPT); }
+    if (j >= ri.beg && j <= ri.end) { hij = __ldcg(rowi + plane_index(ri.beg, ri.end, 0, j)); cij = (unsigned)__ldcg(rowi + plane_index(ri.beg, ri.end, 1, j)); }
     // the first 32 columns left of j in row i (for the F tests), in flight together with the predecessor probes
     int hk0 = inf;
     if ((cur_op & OP_F) && j - 1 - lane >= ri.beg && j - 1 - lane <= ri.end) hk0 = __ldcg(rowi + plane_index(ri.beg, ri.end, 0, j - 1 - lane));
@@ -250,9 +250,8 @@ __device__ int warp_backtrack_step(const RowTables &rt, const DpState &d, const 
         e_in = (cur_op & OP_E) && j >= pin.beg && j <= pin.end;
         if (m_in) pm = __ldcg(prow + plane_index(pin.beg, pin.end, 0, j - 1));
         if (e_in) {
-            const int64_t o = plane_index(pin.beg, pin.end, 0, j);
-            ph = __ldcg(prow + o);
-            const unsigned code = (unsigned)__ldcg(prow + o + CPT);
+            ph = __ldcg(prow + plane_index(pin.beg, pin.end, 0, j));
+            const unsigned code = (unsigned)__ldcg(prow + plane_index(pin.beg, pin.end, 1, j));
             pe1 = e_decode(ph, (int)(code & 0xffffu), inf); pe2 = e_decode(ph, (int)(code >> 16), inf);
         }
     };

@@ -15,14 +15,15 @@
 //     row just computed therefore stay in the owning thread's registers and feed the next row without touching
 //     memory when the predecessor is the previous row (the common case in a near-linear graph); only H[16t-1]
 //     comes from the neighbour thread (warp shuffle; one shared-memory word per warp boundary). Predecessors
-//     further back are read from the planes in global memory (L2), coalesced 16 B per thread;
+//     further back are read from the planes in global memory (L2), one 16-byte chunk per thread and instruction, a warp's
+//     chunk 512 contiguous bytes;
 //   * the max-plus recurrence of the two insertion states F1/F2 along the row is turned into a plain prefix
 //     maximum by the substitution A[k] = H'[k] - oe + (k+1)*e  =>  F[j] = max_{k<j} A[k] - j*e: 16 serial cells per
 //     thread, a warp shuffle scan over the 32 thread aggregates, a redux over the warp aggregates staged in
 //     shared memory;
 //   * per cell the sweep writes 8 bytes for the traceback and for later rows -- H (int32) and the two E values as 16-bit
 //     distances below H; F1 / F2 are not stored, the traceback recomputes the few row prefixes it needs
-//     (poa_types.h: DpState) -- in a thread-blocked layout where each thread writes whole 32-byte sectors:
+//     (poa_types.h: DpState) -- in a chunk-major layout where every 128-bit warp store writes 512 contiguous bytes:
 //     8 B/cell of HBM write traffic (the reference streams five int32 planes, 20 B/cell) is the kernel's only DRAM stream;
 //   * two block barriers per row.
 // Integer DP: no tensor cores. int32 everywhere with the reference's own "minus infinity" so that finite cells
@@ -43,24 +44,22 @@ struct KShared {
     int smat[5 * 8];       // [graph base][query code 0..4, 5 = "no base": column 0 / beyond the query -> 0]
     int wF[2][2][32];      // [row parity][plane F1/F2][warp] block scan staging
     int wM[2][4][32];      // [row parity][max, leftmost, rightmost, H of the warp's last column][warp]
+    RowRec rec[2];         // [row parity] the sweep's row record, fetched one row ahead
 };
 
 __device__ __forceinline__ int4 ld4cg(const int *p) { return __ldcg(reinterpret_cast<const int4 *>(p)); }
 __device__ __forceinline__ void st4(int *p, int a, int b, int c, int d) { *reinterpret_cast<int4 *>(p) = make_int4(a, b, c, d); }
 __device__ __forceinline__ int max3(int a, int b, int c) { return max(max(a, b), c); }
-// One whole 32-byte sector per thread, as two back-to-back 128-bit global accesses (sm_90 has no 256-bit LDG/STG). The two
-// halves of a sector are issued by consecutive instructions, so they are expected to reach L2 close together; that has not been
-// measured on sm_90. p must be 32-byte aligned
-__device__ __forceinline__ void st8(int *p, int a0, int a1, int a2, int a3, int a4, int a5, int a6, int a7) {
-    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.v4.b32 [%0+16], {%5,%6,%7,%8};"
-                 ::"l"(p), "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(a4), "r"(a5), "r"(a6), "r"(a7) : "memory");
+// 16-byte global -> shared copy that bypasses the registers (completes at cp_async_wait_all)
+__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
-struct int8v { int v[8]; };
-__device__ __forceinline__ int8v ld8cg(const int *p) {
-    int8v r;
-    asm volatile("ld.global.cg.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.cg.v4.b32 {%4,%5,%6,%7}, [%8+16];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7]) : "l"(p) : "memory");
-    return r;
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// a padding block of a stored row (poa_types.h: DpState): the out-of-band values H = inf_min, D = 0, so that every sector the
+// warp writes is whole. tp: the block's chunk 0, cs: ints between chunks
+__device__ __forceinline__ void store_pad(int *tp, int64_t cs, int NEG) {
+#pragma unroll
+    for (int c = 0; c < TB / CHUNK; ++c) st4(tp + c * cs, c < CPT / CHUNK ? NEG : 0, c < CPT / CHUNK ? NEG : 0, c < CPT / CHUNK ? NEG : 0, c < CPT / CHUNK ? NEG : 0);
 }
 
 
@@ -89,15 +88,15 @@ __device__ __forceinline__ void row_pass1(int (&H)[CPT], int (&E1)[CPT], int (&E
 // and the traceback never reads the F planes outside the band, so only H / E1 / E2 are forced (they feed later rows).
 template <int MODE>
 __device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], int P1, int P2, int j0, int beg, int end, int NEG,
-                                          int je1, int je2, int e1, int e2, int o1, int o2, int *tp, int &tmax) {
+                                          int je1, int je2, int e1, int e2, int o1, int o2, int *tp, int64_t cs, int &tmax) {
     const int oe1 = o1 + e1, oe2 = o2 + e2;
-    // (each st8 writes one whole 32-byte sector)
+    // one H chunk and one D chunk per 4 cells (tp: the thread's chunk 0, cs: ints between chunks; poa_types.h: DpState)
 #pragma unroll
-    for (int oc = 0; oc < 2; ++oc) {
-        int dd[8];
+    for (int oc = 0; oc < CPT / CHUNK; ++oc) {
+        int dd[CHUNK];
 #pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            const int e = oc * 8 + u, u1 = je1 + e * e1, u2 = je2 + e * e2;
+        for (int u = 0; u < CHUNK; ++u) {
+            const int e = oc * CHUNK + u, u1 = je1 + e * e1, u2 = je2 + e * e2;
             const int f1 = P1 - o1 - u1, f2 = P2 - o2 - u2;                // F[j] = max_{k<j} A'[k] - o - j*e (used, not stored)
             P1 = __viaddmax_s32(H[e], u1, P1); P2 = __viaddmax_s32(H[e], u2, P2);
             int h = __vimax3_s32(H[e], f1, f2);                            // :1067
@@ -114,11 +113,9 @@ __device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E
             dd[u] = (h - x1) | ((h - x2) << 16);                           // e <= H - E' <= oe < 65535 (0 outside the band)
             tmax = max(tmax, h);
         }
-        st8(tp + CPT + oc * 8, dd[0], dd[1], dd[2], dd[3], dd[4], dd[5], dd[6], dd[7]);
+        st4(tp + oc * cs, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
+        st4(tp + (CPT / CHUNK + oc) * cs, dd[0], dd[1], dd[2], dd[3]);
     }
-#pragma unroll
-    for (int oc = 0; oc < 2; ++oc)
-        st8(tp + oc * 8, H[oc * 8], H[oc * 8 + 1], H[oc * 8 + 2], H[oc * 8 + 3], H[oc * 8 + 4], H[oc * 8 + 5], H[oc * 8 + 6], H[oc * 8 + 7]);
 }
 
 // left/right-most column of the thread's cells that attain v (only in-band cells count)
@@ -138,7 +135,7 @@ __device__ __forceinline__ void row_argmax(const int (&H)[CPT], int v, int j0, i
 // banded convex-gap DP of query q[1..L] against the sorted graph. All threads of the CTA; L + 1 <= 16 * blockDim.x.
 // Returns the number of banded cells (sum of dp_end-dp_beg+1), or -1 if the planes outgrew the slot.
 // ---------------------------------------------------------------------------------------------------------
-__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L) {
+__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L, uint2 *qsm) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const PoaParams &P = A.P;
     // slot arrays addressed from the kernel parameters (not through the pointers cached in shared memory), so that the
@@ -166,6 +163,9 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         const uint32_t c = (j >= 1 && j <= L) ? qg[j - 1] : 5u;
         qc[e >> 3] |= c << ((e & 7) * 4);
     }
+    // they are read back from shared memory in every row (only by this thread): kept in registers across the row loop, they let
+    // the compiler hoist 16 per-column table offsets out of it, which then spill
+    qsm[tid] = make_uint2(qc[0], qc[1]);
 
     int H[CPT], E1[CPT], E2[CPT];          // the previous row's values of my columns (valid iff prev_active)
     bool prev_active;
@@ -176,38 +176,39 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
     {
         const int dd = L - rec_tab[0].rd;
         prev_end = min(L, max(0, dd) + w);
-        const int nT = prev_end / CPT + 1;
-        if ((int64_t)nT * TB > plane_cap) return -1;
+        const int nT = prev_end / CPT + 1, nTs = row_blocks(0, prev_end);
+        if ((int64_t)nTs * TB > plane_cap) return -1;
         prev_active = tid < nT;
-        if (prev_active) {
-            int *tp = planes + tid * TB;
-            int dd[CPT];
+        // the threads past the band (the padding block among them) hold out-of-band values
+        int D[CPT];
 #pragma unroll
-            for (int e = 0; e < CPT; ++e) {
-                const int j = j0 + e;
-                if (j == 0) { H[e] = 0; E1[e] = -oe1; E2[e] = -oe2; dd[e] = oe1 | (oe2 << 16); }
-                else if (j <= prev_end) { H[e] = max(-P.o1 - e1 * j, -P.o2 - e2 * j); E1[e] = NEG; E2[e] = NEG; dd[e] = E_NEG16 | (E_NEG16 << 16); }
-                else { H[e] = E1[e] = E2[e] = NEG; dd[e] = 0; }
-            }
-#pragma unroll
-            for (int oc = 0; oc < 2; ++oc) {
-                st8(tp + oc * 8, H[oc * 8], H[oc * 8 + 1], H[oc * 8 + 2], H[oc * 8 + 3], H[oc * 8 + 4], H[oc * 8 + 5], H[oc * 8 + 6], H[oc * 8 + 7]);
-                st8(tp + CPT + oc * 8, dd[oc * 8], dd[oc * 8 + 1], dd[oc * 8 + 2], dd[oc * 8 + 3], dd[oc * 8 + 4], dd[oc * 8 + 5], dd[oc * 8 + 6], dd[oc * 8 + 7]);
-            }
-        } else {
-#pragma unroll
-            for (int e = 0; e < CPT; ++e) H[e] = E1[e] = E2[e] = NEG;
+        for (int e = 0; e < CPT; ++e) {
+            const int j = j0 + e;
+            if (j == 0) { H[e] = 0; E1[e] = -oe1; E2[e] = -oe2; D[e] = oe1 | (oe2 << 16); }
+            else if (j <= prev_end) { H[e] = max(-P.o1 - e1 * j, -P.o2 - e2 * j); E1[e] = NEG; E2[e] = NEG; D[e] = E_NEG16 | (E_NEG16 << 16); }
+            else { H[e] = E1[e] = E2[e] = NEG; D[e] = 0; }
         }
-        if (lane == 31) S.wM[0][3][warp] = prev_active ? H[CPT - 1] : NEG;
+        if (tid < nTs) {
+            int *tp = planes + chunk_index(nTs, tid, 0);
+            const int64_t cs = chunk_index(nTs, 0, 1);
+#pragma unroll
+            for (int oc = 0; oc < CPT / CHUNK; ++oc) {
+                st4(tp + oc * cs, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
+                st4(tp + (CPT / CHUNK + oc) * cs, D[oc * CHUNK], D[oc * CHUNK + 1], D[oc * CHUNK + 2], D[oc * CHUNK + 3]);
+            }
+        }
+        if (lane == 31) S.wM[0][3][warp] = H[CPT - 1];
         if (tid == 0) { RowInfo ri; ri.beg = 0; ri.end = prev_end; ri.left = 0; ri.right = 0; info[0] = ri; row_off[0] = 0; }
-        cur_blk = nT; cells = prev_end + 1;
+        cur_blk = nTs; cells = prev_end + 1;
+        if (tid == 0) { cp_async16(&S.rec[1], rec_tab + (R > 1 ? 1 : 0)); cp_async_wait_all(); }
     }
     __syncthreads();
 
-    RowRec rec = rec_tab[R > 1 ? 1 : 0];
     for (int r = 1; r < R; ++r) {
         const int par = r & 1;
-        const RowRec nrec = rec_tab[r + 1 < R ? r + 1 : r];      // next row's record, in flight while this row computes
+        const RowRec rec = S.rec[par];
+        // the next row's record, in flight while this row computes (its buffer was last read two barriers ago)
+        if (tid == 0 && r + 1 < R) cp_async16(&S.rec[par ^ 1], rec_tab + r + 1);
         // ---- band of the row (GET_AD_DP_BEGIN/END + lane-group snap, :946-960) ----
         const int b = rec.base_npre & 0xff, npre = rec.base_npre >> 8;
         const int dd = L - rec.rd;
@@ -230,7 +231,8 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         const int end = min(L, max(maxR, dd) + w);
         if ((beg >> pn_shift) < (min_pre_beg >> pn_shift)) beg = min_pre_beg;
         const int t0 = beg >> 4, nT = (end >> 4) - t0 + 1, tt = tid - t0;
-        if ((int64_t)(cur_blk + nT) * TB > plane_cap) return -1;        // uniform across the CTA
+        const int nTs = row_blocks(beg, end), tts = tid - row_t0(beg);   // stored blocks, my stored block (poa_types.h: DpState)
+        if ((int64_t)(cur_blk + nTs) * TB > plane_cap) return -1;       // uniform across the CTA
         const bool active = tt >= 0 && tt < nT;
         // masking is decided per WARP (no divergent double execution): 0 = all active threads inside the band,
         // 1 = some columns left of the band, 2 = some columns right of it only
@@ -260,25 +262,30 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
                 const int p = k == 0 ? rec.pre0 : pre_row[rec.pre_off + k];
                 if (p == r - 1) continue;
                 const RowInfo pi = info[p];
-                const int pt0 = pi.beg >> 4, pnT = (pi.end >> 4) - pt0 + 1, ptt = tid - pt0;
-                const int *Hp = planes + row_off[p] + (int64_t)ptt * TB;      // my block of row p (if stored)
+                const int pt0 = pi.beg >> 4, pnT = (pi.end >> 4) - pt0 + 1, ptt = tid - pt0, pnTs = row_blocks(pi.beg, pi.end);
+                const int *Hp = planes + row_off[p] + chunk_index(pnTs, tid - row_t0(pi.beg), 0);   // my block of row p (if stored)
+                const int64_t pcs = chunk_index(pnTs, 0, 1);
                 if (ptt >= 0 && ptt < pnT) {
 #pragma unroll
-                    for (int oc = 0; oc < 2; ++oc) {
-                        const int8v h = ld8cg(Hp + oc * 8), dv = ld8cg(Hp + CPT + oc * 8);
+                    for (int oc = 0; oc < CPT / CHUNK; ++oc) {
+                        const int4 h4 = ld4cg(Hp + oc * pcs), d4 = ld4cg(Hp + (CPT / CHUNK + oc) * pcs);
+                        const int h[CHUNK] = {h4.x, h4.y, h4.z, h4.w}, dv[CHUNK] = {d4.x, d4.y, d4.z, d4.w};
 #pragma unroll
-                        for (int u = 0; u < 8; ++u) {
-                            const int e = oc * 8 + u;
-                            const int c1 = dv.v[u] & 0xffff, c2 = (int)((unsigned)dv.v[u] >> 16);
-                            if (e + 1 < CPT) H[e + 1] = max(H[e + 1], h.v[u]);
-                            E1[e] = max(E1[e], c1 == E_NEG16 ? NEG : h.v[u] - c1); E2[e] = max(E2[e], c2 == E_NEG16 ? NEG : h.v[u] - c2);
+                        for (int u = 0; u < CHUNK; ++u) {
+                            const int e = oc * CHUNK + u;
+                            const int c1 = dv[u] & 0xffff, c2 = (int)((unsigned)dv[u] >> 16);
+                            if (e + 1 < CPT) H[e + 1] = max(H[e + 1], h[u]);
+                            E1[e] = max(E1[e], c1 == E_NEG16 ? NEG : h[u] - c1); E2[e] = max(E2[e], c2 == E_NEG16 ? NEG : h[u] - c2);
                         }
                     }
                 }
-                if (ptt >= 1 && ptt <= pnT) H[0] = max(H[0], __ldcg(Hp - TB + CPT - 1));    // H[16*tid - 1]: last H of the left neighbour's block
+                // H[16*tid - 1]: the last H (chunk 3) of the left neighbour's block
+                if (ptt >= 1 && ptt <= pnT) H[0] = max(H[0], __ldcg(Hp - CHUNK + (CPT / CHUNK - 1) * pcs + CHUNK - 1));
             }
-            if (wmode != 1) row_pass1<false>(H, E1, E2, mrow, qc, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
-            else row_pass1<true>(H, E1, E2, mrow, qc, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
+            const uint2 q2 = qsm[tid];
+            const uint32_t qr[2] = {q2.x, q2.y};
+            if (wmode != 1) row_pass1<false>(H, E1, E2, mrow, qr, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
+            else row_pass1<true>(H, E1, E2, mrow, qr, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
         }
         // ---- exclusive prefix maximum over the row: warp shuffle scan + redux over warp aggregates ----
         int inc1 = agg1, inc2 = agg2;
@@ -297,11 +304,14 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
             P1 = max(__reduce_max_sync(FULL, wv1), ex1); P2 = max(__reduce_max_sync(FULL, wv2), ex2);
         }
         int tmax = NEG - 1000;
-        if (active) {
-            int *tp = planes + (int64_t)(cur_blk + tt) * TB;
-            if (wmode == 0) row_pass2<0>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, tmax);
-            else if (wmode == 2) row_pass2<2>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, tmax);
-            else row_pass2<1>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, tmax);
+        {
+            int *tp = planes + (int64_t)cur_blk * TB + chunk_index(nTs, tts, 0);
+            const int64_t cs = chunk_index(nTs, 0, 1);
+            if (active) {
+                if (wmode == 0) row_pass2<0>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
+                else if (wmode == 2) row_pass2<2>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
+                else row_pass2<1>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
+            } else if ((unsigned)tts < (unsigned)nTs) store_pad(tp, cs, NEG);
         }
         // ---- left/right-most argmax of H over the band (simd_abpoa_max_in_row, :1107-1119) ----
         {
@@ -314,6 +324,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
             if (lane == 0) { S.wM[par][0][warp] = wmax; S.wM[par][1][warp] = wl; S.wM[par][2][warp] = wr; }
             if (lane == 31) S.wM[par][3][warp] = active ? H[CPT - 1] : NEG;
         }
+        if (tid == 0) cp_async_wait_all();
         __syncthreads();
         {
             const int v = lane < nwarps ? S.wM[par][0][lane] : NEG - 1000;
@@ -324,8 +335,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         }
         prev_beg = beg; prev_end = end; prev_active = active;
         if (tid == 0) { RowInfo ri; ri.beg = beg; ri.end = end; ri.left = prev_left; ri.right = prev_right; info[r] = ri; row_off[r] = (int64_t)cur_blk * TB; }
-        cur_blk += nT; cells += end - beg + 1;
-        rec = nrec;
+        cur_blk += nTs; cells += end - beg + 1;
     }
     __syncthreads();
     return cells;
@@ -353,9 +363,11 @@ __device__ __forceinline__ void carve(KShared &S, const BatchArgs &A, int slot) 
 
 #define PHASE_TICK(ph) do { if (A.phase_clk && threadIdx.x == 0) { unsigned long long _n = clock64(); A.phase_clk[(size_t)blockIdx.x * PH_N + (ph)] += _n - t_last; t_last = _n; } } while (0)
 
+template <int NT>
 __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
     extern __shared__ __align__(16) unsigned char dyn_smem[];    // scratch of the topological sort (poa_cta.cuh)
     __shared__ KShared S;
+    __shared__ uint2 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
     const int tid = threadIdx.x;
     int *ws = &S.wF[0][0][0];
     if (tid == 0) carve(S, A, blockIdx.x);
@@ -394,7 +406,7 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
                 PHASE_TICK(PH_FUSE);
             } else {
                 long long c = -2;
-                if (L + 1 <= CPT * (int)blockDim.x) c = dp_sweep(S, A, q, L);
+                if (L + 1 <= CPT * (int)blockDim.x) c = dp_sweep(S, A, q, L, qsm);
                 if (c < 0) { if (tid == 0) S.g.err = c == -2 ? JOB_ERR_QUERY_LEN : JOB_ERR_PLANE_CAP; c = 0; }
                 cells += c;
                 __syncthreads();
@@ -441,14 +453,14 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
 //   queries up to 511 bases -> one warp, 16 CTAs per SM;  up to 1023 -> 64 threads;
 //   up to 2047 -> 128 threads, 4 CTAs per SM;  up to 4095 -> 256 threads, 2 per SM;
 //   up to 10239 (covers Cactus' 10 kbp window) -> 640 threads;  up to 16383 -> 1024 threads.
-extern "C" __global__ void __launch_bounds__(32, 16) poa_msa_kernel_t32(const BatchArgs A) { poa_msa_body(A); }
-extern "C" __global__ void __launch_bounds__(64, 8) poa_msa_kernel_t64(const BatchArgs A) { poa_msa_body(A); }
+extern "C" __global__ void __launch_bounds__(32, 16) poa_msa_kernel_t32(const BatchArgs A) { poa_msa_body<32>(A); }
+extern "C" __global__ void __launch_bounds__(64, 8) poa_msa_kernel_t64(const BatchArgs A) { poa_msa_body<64>(A); }
 #ifndef BARB200_T128_MINB
 #define BARB200_T128_MINB 4
 #endif
-extern "C" __global__ void __launch_bounds__(128, BARB200_T128_MINB) poa_msa_kernel_t128(const BatchArgs A) { poa_msa_body(A); }
-extern "C" __global__ void __launch_bounds__(256, 2) poa_msa_kernel_t256(const BatchArgs A) { poa_msa_body(A); }
-extern "C" __global__ void __launch_bounds__(640, 1) poa_msa_kernel_t640(const BatchArgs A) { poa_msa_body(A); }
-extern "C" __global__ void __launch_bounds__(1024, 1) poa_msa_kernel_t1024(const BatchArgs A) { poa_msa_body(A); }
+extern "C" __global__ void __launch_bounds__(128, BARB200_T128_MINB) poa_msa_kernel_t128(const BatchArgs A) { poa_msa_body<128>(A); }
+extern "C" __global__ void __launch_bounds__(256, 2) poa_msa_kernel_t256(const BatchArgs A) { poa_msa_body<256>(A); }
+extern "C" __global__ void __launch_bounds__(640, 1) poa_msa_kernel_t640(const BatchArgs A) { poa_msa_body<640>(A); }
+extern "C" __global__ void __launch_bounds__(1024, 1) poa_msa_kernel_t1024(const BatchArgs A) { poa_msa_body<1024>(A); }
 
 }  // namespace barb200

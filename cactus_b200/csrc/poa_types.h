@@ -99,10 +99,13 @@ struct alignas(16) RowInfo {
 
 // Banded DP planes of the current alignment.
 // Column ownership is fixed: thread t of the CTA owns columns [CPT*t, CPT*t + CPT) of EVERY row, so the values of the
-// previous row stay in that thread's registers. A row with band [beg, end] is stored for the threads
-// t0 = beg/CPT .. t1 = end/CPT only (nT = t1-t0+1), at planes + row_off[r], "thread-major": thread t's block of
-// TB = 2*CPT ints = [H(16) | D(16)] sits at int offset (t-t0)*TB; a thread writes its 128 bytes of a row as four
-// whole 32 B sectors at immediate offsets from one pointer (a warp covers one contiguous 4 KB run).
+// previous row stay in that thread's registers. A row with band [beg, end] covers the threads t0 = beg/CPT .. t1 = end/CPT
+// and is stored at planes + row_off[r] as row_blocks(beg, end) thread blocks of TB = 2*CPT ints, starting at thread
+// row_t0(beg): the stored range is widened to an even first thread and an even count, so that it has at most one
+// padding block at either end (written with out-of-band values, never read). The row is "chunk-major": 8 chunk planes of
+// 4 ints each -- H columns 0-3, 4-7, 8-11, 12-15 of every block, then the same four for D -- and stored block b's chunk c
+// sits at int offset (c * nblk + b) * 4. A warp's 128-bit access to one chunk thus covers 512 contiguous bytes, and the even
+// start and count keep every such run 32 B aligned (whole sectors only).
 //
 // What is stored, and why it is enough for the reference's traceback (abpoa_align_simd.c:309-458) -- 8 bytes per cell
 // instead of the reference's five int32 planes (20 bytes):
@@ -127,13 +130,18 @@ struct DpState {
     int fc_cap, fc_row, fc_hi;          // columns per plane; cached row (-1: none) and its highest computed column
 };
 
-// int offset of column j of `plane` (0: H, 1: D) inside the row's block (see DpState); j must lie in a stored thread's range
+// Row layout (see DpState). j must lie in a stored thread's range.
 constexpr int TB = 2 * CPT;   // ints per thread block of a row
+constexpr int CHUNK = 4;      // ints per chunk (one 128-bit access)
+HD int row_t0(int beg) { return (beg / CPT) & ~1; }                                   // first stored thread
+HD int row_blocks(int beg, int end) { return ((end / CPT - row_t0(beg)) | 1) + 1; }   // stored blocks (even)
+// int offset of chunk c (0-3: H, 4-7: D) of stored block b in a row of nblk blocks
+HD int64_t chunk_index(int nblk, int b, int c) { return ((int64_t)c * nblk + b) * CHUNK; }
+// int offset of column j of `plane` (0: H, 1: D) inside the row
 HD int64_t plane_index(int beg, int end, int plane, int j) {
-    (void)end;
-    return (int64_t)(j / CPT - beg / CPT) * TB + plane * CPT + j % CPT;
+    return chunk_index(row_blocks(beg, end), j / CPT - row_t0(beg), plane * (CPT / CHUNK) + j % CPT / CHUNK) + j % CHUNK;
 }
-HD int64_t row_ints(int beg, int end) { return (int64_t)TB * (end / CPT - beg / CPT + 1); }
+HD int64_t row_ints(int beg, int end) { return (int64_t)TB * row_blocks(beg, end); }
 // E value from H and its 16-bit distance code
 HD int e_decode(int h, int code, int inf_min) { return code == E_NEG16 ? inf_min : h - code; }
 HD int e_encode(int h, int e) { const int d = h - e; return (d >= 0 && d < E_NEG16) ? d : E_NEG16; }
