@@ -303,7 +303,11 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
             const int wv1 = lane < warp ? S.wF[par][0][lane] : id1, wv2 = lane < warp ? S.wF[par][1][lane] : id2;
             P1 = max(__reduce_max_sync(FULL, wv1), ex1); P2 = max(__reduce_max_sync(FULL, wv2), ex2);
         }
-        int tmax = NEG - 1000;
+        // the row maximum starts below every value a cell can hold. Not inf_min minus a constant: inf_min lies only
+        // max(min_mis, o1 + e1, o2 + e2) + 512 * max(e1, e2) above INT32_MIN, which wraps for extensions of at most 1. The reference
+        // counts only cells above inf_min (simd_abpoa_max_in_row); every row a band reaches has one (a predecessor's argmax column or
+        // the one right of it), so both find the same maximum
+        int tmax = INT32_MIN;
         {
             int *tp = planes + (int64_t)cur_blk * TB + chunk_index(nTs, tts, 0);
             const int64_t cs = chunk_index(nTs, 0, 1);
@@ -327,7 +331,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         if (tid == 0) cp_async_wait_all();
         __syncthreads();
         {
-            const int v = lane < nwarps ? S.wM[par][0][lane] : NEG - 1000;
+            const int v = lane < nwarps ? S.wM[par][0][lane] : INT32_MIN;       // lanes without a warp: below every maximum
             const int bmax = __reduce_max_sync(FULL, v);
             const int l = (lane < nwarps && v == bmax) ? S.wM[par][1][lane] : 0x7fffffff;
             const int rr = (lane < nwarps && v == bmax) ? S.wM[par][2][lane] : -1;

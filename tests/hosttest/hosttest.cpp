@@ -35,7 +35,8 @@ static long long emulate_sweep(const Graph &g, const RowTables &rt, DpState &d, 
         }
         if (cur_off + row_ints(beg, end) > d.plane_cap) return -1;
         int *rowp = d.planes + cur_off;
-        int P1 = NEG + beg * e1, P2 = NEG + beg * e2, tmax = NEG - 1000, tl = 0, tr = r == 0 ? 0 : -1;
+        // the row maximum starts below every value, as in the kernel (inf_min minus a constant wraps when both extensions are <= 1)
+        int P1 = NEG + beg * e1, P2 = NEG + beg * e2, tmax = INT32_MIN, tl = 0, tr = r == 0 ? 0 : -1;
         for (int j = beg / CPT * CPT; j <= (end / CPT) * CPT + CPT - 1; ++j) {
             int h, x1, x2, f1, f2;
             if (r == 0) {
@@ -68,6 +69,10 @@ static long long emulate_sweep(const Graph &g, const RowTables &rt, DpState &d, 
             (void)f1; (void)f2;
             rowp[plane_index(beg, end, 0, j)] = h; rowp[plane_index(beg, end, 1, j)] = c1 | (c2 << 16);
         }
+        // the reference counts only cells above inf_min as a row maximum (simd_abpoa_max_in_row starts at inf_min), the kernel every
+        // cell. They agree because every row a band reaches has a cell above inf_min (the band holds a predecessor's argmax column
+        // or the one right of it), which this emulation asserts
+        if (r > 0 && tmax <= NEG) return -2;
         RowInfo ri; ri.beg = beg; ri.end = end; ri.left = r == 0 ? 0 : tl; ri.right = r == 0 ? 0 : tr;
         d.info[r] = ri; d.row_off[r] = cur_off;
         cur_off += row_ints(beg, end); cells += end - beg + 1;

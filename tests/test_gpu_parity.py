@@ -20,14 +20,15 @@ def engine():
     e.close()
 
 
-def engine_for(params):
+def engine_for(params, **engine_knobs):
+    """an Engine with the oracle's parameters (R.params_dict) and optional engine knobs (threads_per_block, ...)"""
     import cactus_b200 as cb
     return cb.Engine(cb.PoaParams(
         partialOrderAlignmentBandConstant=params["wb"], partialOrderAlignmentBandFraction=params["wf"],
         partialOrderAlignmentGapOpenPenalty1=params["o1"], partialOrderAlignmentGapExtensionPenalty1=params["e1"],
         partialOrderAlignmentGapOpenPenalty2=params["o2"], partialOrderAlignmentGapExtensionPenalty2=params["e2"],
         partialOrderAlignmentMinimizerK=params["k"], partialOrderAlignmentMinimizerW=params["w"],
-        partialOrderAlignmentMinimizerMinW=params["min_w"], partialOrderAlignmentProgressiveMode=params["progressive"]))
+        partialOrderAlignmentMinimizerMinW=params["min_w"], partialOrderAlignmentProgressiveMode=params["progressive"], **engine_knobs))
 
 
 def test_golden_poa(engine):
@@ -96,10 +97,13 @@ def test_narrow_band_params(oracle_built):
         e.close()
 
 
-@pytest.mark.parametrize("gaps", [(400, 30, 1200, 1), (4, 2, 24, 1), (400, 30, 1200, 30), (1200, 1, 400, 30), (400, 30, 300, 1), (6, 2, 6, 2)])
+@pytest.mark.parametrize("gaps", [(400, 30, 1200, 1), (4, 2, 24, 1), (400, 30, 1200, 30), (1200, 1, 400, 30), (400, 30, 300, 1), (6, 2, 6, 2),
+                                  (4, 1, 24, 1), (1, 1, 1, 1), (2, 1, 30, 0)])
 def test_long_gaps_and_gap_models(oracle_built, gaps):
     """block indels of 1..300 bases under Cactus' penalties, abPOA's defaults, equal extensions, swapped gap pairs, a second gap
-    that is cheaper everywhere, and two identical gaps: the insertion scan's crossover bound in every regime"""
+    that is cheaper everywhere, and two identical gaps: the insertion scan's crossover bound in every regime. The models with
+    extensions of at most 1 put the reference's minus infinity within a few hundred of INT32_MIN (the row maximum's seed must not
+    wrap there), and (2, 1, 30, 0) has a gap that costs nothing to extend"""
     o1, e1, o2, e2 = gaps
     rng = np.random.default_rng(4242 + o1 + 7 * e2)
     p = R.cactus_params(o1=o1, e1=e1, o2=o2, e2=e2, wb=300, wf=0.05)
@@ -195,6 +199,8 @@ def test_errors_are_loud(engine):
         engine.poa_msa_batch([[np.array([0, 1, 7], np.uint8), np.array([0, 1], np.uint8)]])
     with pytest.raises(cb.BarB200Error):
         engine.poa_msa_batch([[np.array([], np.uint8), np.array([0, 1], np.uint8)]])
+    with pytest.raises(cb.BarB200Error):            # one base past the largest CTA class (1024 threads x 16 columns - 1)
+        engine.poa_msa_batch([[np.zeros(16384, np.uint8), np.array([0, 1], np.uint8)]])
     with pytest.raises(cb.BarB200Error):
         cb.Engine(cb.PoaParams(partialOrderAlignmentGapOpenPenalty2=0))
 

@@ -35,18 +35,30 @@ def test_hosttest_random_vs_oracle(oracle_built):
         assert_same_trace(R.oracle_poa_msa_trace(seqs, p), R.hosttest_poa_msa_trace(seqs, p), (it, K, L, kw))
 
 
-def test_traceback_rule_without_f_planes_many_gap_models():
+def test_traceback_rule_without_f_planes_many_gap_models(oracle_built):
     """the warp traceback's rule (insertions whole, from the row's H values; F1 only within the convex crossover distance), stated
     serially, runs in lock step with the reference's rule inside the host build's traceback (poa_graph.cuh: dp_backtrack) and fails the
-    job on any disagreement: a few hundred alignments with block indels under random convex gap penalties of every ordering"""
+    job on any disagreement: a few hundred alignments with block indels under random convex gap penalties of every ordering, each
+    equal to the oracle's. Extensions of 0 and 1 are drawn often: with both at most 1 the reference's minus infinity lies within a few
+    hundred of INT32_MIN"""
     rng = np.random.default_rng(2024)
-    fixed = [(400, 30, 1200, 1), (4, 2, 24, 1), (10, 3, 10, 3), (50, 1, 3, 9), (7, 5, 100, 5), (300, 2, 20, 40), (1, 1, 1, 1)]
+    fixed = [(400, 30, 1200, 1), (4, 2, 24, 1), (10, 3, 10, 3), (50, 1, 3, 9), (7, 5, 100, 5), (300, 2, 20, 40), (1, 1, 1, 1),
+             (4, 1, 24, 1), (2, 1, 30, 0), (400, 0, 1200, 1)]
+
+    def ext():
+        return int(rng.choice([0, 1, int(rng.integers(2, 40))]))
+
     for it in range(60):
-        o1, e1, o2, e2 = fixed[it] if it < len(fixed) else (int(rng.integers(1, 600)), int(rng.integers(1, 40)), int(rng.integers(1, 1500)), int(rng.integers(1, 40)))
+        if it < len(fixed):
+            o1, e1, o2, e2 = fixed[it]
+        else:
+            o1, e1, o2, e2 = int(rng.integers(1, 600)), ext(), int(rng.integers(1, 1500)), ext()
+            if e1 == 0 and e2 == 0:             # barb200_create requires one extension > 0
+                e2 = 1
         p = R.cactus_params(o1=o1, e1=e1, o2=o2, e2=e2, wb=int(rng.choice([20, 100, 1000])), wf=0.05)
         seqs = gapped_family(rng, int(rng.integers(2, 7)), int(rng.choice([40, 150, 400])), [1, 2, 3, 5, 9, 20, 27, 28, 33, 64, 90])
         tr = R.hosttest_poa_msa_trace(seqs, p)           # asserts job status 0
-        assert tr["msa"].shape[0] == len(seqs)
+        assert_same_trace(R.oracle_poa_msa_trace(seqs, p), tr, (it, (o1, e1, o2, e2), p.wb))
 
 
 def test_hosttest_unrelated_ragged(oracle_built):

@@ -45,10 +45,12 @@ def test_poa_msa_trace_random_families(oracle_built, seed):
         same_trace("random_families/%d/%d" % (seed, it), R.oracle_poa_msa_trace(seqs, p), seqs, p)
 
 
-@pytest.mark.parametrize("gaps", [(400, 30, 1200, 1), (4, 2, 24, 1), (400, 30, 1200, 30), (1200, 1, 400, 30), (400, 30, 300, 1), (6, 2, 6, 2)])
+@pytest.mark.parametrize("gaps", [(400, 30, 1200, 1), (4, 2, 24, 1), (400, 30, 1200, 30), (1200, 1, 400, 30), (400, 30, 300, 1), (6, 2, 6, 2),
+                                  (4, 1, 24, 1), (1, 1, 1, 1), (2, 1, 30, 0)])
 def test_poa_msa_long_gaps_and_gap_models(oracle_built, gaps):
     """the inputs of test_gpu_parity.py::test_long_gaps_and_gap_models: the oracle (and the serial traceback the host build runs)
-    against the reference, so that the GPU test's checker is pinned in these regimes too"""
+    against the reference, so that the GPU test's checker is pinned in these regimes too. The last three models have extensions of
+    at most 1 (and one of 0), where the reference's minus infinity lies only a few hundred above INT32_MIN"""
     o1, e1, o2, e2 = gaps
     rng = np.random.default_rng(4242 + o1 + 7 * e2)
     p = R.cactus_params(o1=o1, e1=e1, o2=o2, e2=e2, wb=300, wf=0.05)
