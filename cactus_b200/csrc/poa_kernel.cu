@@ -48,7 +48,13 @@ struct KShared {
 };
 
 __device__ __forceinline__ int4 ld4cg(const int *p) { return __ldcg(reinterpret_cast<const int4 *>(p)); }
-__device__ __forceinline__ void st4(int *p, int a, int b, int c, int d) { *reinterpret_cast<int4 *>(p) = make_int4(a, b, c, d); }
+// one 128-bit store per plane chunk: a warp's store writes 512 contiguous bytes, 4 whole lines, in one instruction. An int4
+// assignment is split into four 32-bit stores by NVVM in this kernel, and each of those spans the same 4 lines. The PTX store
+// keeps the default cache policy: far-predecessor rows are read back from L2 a few rows after they are written.
+// tests/test_sweep_sass.py pins every store of this helper to STG.E.128
+__device__ __forceinline__ void st4(int *p, int a, int b, int c, int d) {
+    asm volatile("st.global.v4.s32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
 __device__ __forceinline__ int max3(int a, int b, int c) { return max(max(a, b), c); }
 // 16-byte global -> shared copy that bypasses the registers (completes at cp_async_wait_all)
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
@@ -110,7 +116,7 @@ __device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E
                 h = inb ? h : NEG; x1 = inb ? x1 : NEG; x2 = inb ? x2 : NEG;
             }
             H[e] = h; E1[e] = x1; E2[e] = x2;
-            dd[u] = (h - x1) | ((h - x2) << 16);                           // e <= H - E' <= oe < 65535 (0 outside the band)
+            dd[u] = __byte_perm(h - x1, h - x2, 0x5410);                  // (h-x1) | (h-x2) << 16: e <= H - E' <= oe < 65535 (0 outside the band)
             tmax = max(tmax, h);
         }
         st4(tp + oc * cs, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
