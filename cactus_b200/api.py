@@ -167,6 +167,9 @@ class PoaParams:
             mat = [int(v) for v in mat.split()]
         if len(mat) != 25:
             raise ValueError("partialOrderAlignmentSubMatrix needs 25 values")
+        if any(not -2 ** 31 <= int(v) < 2 ** 31 for v in mat):
+            # a C int would wrap such a value, possibly into the range barb200_create accepts
+            raise ValueError("partialOrderAlignmentSubMatrix values must fit a 32-bit int")
         c = _CParams()
         for i, v in enumerate(mat):
             c.mat[i] = int(v)

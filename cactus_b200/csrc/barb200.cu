@@ -250,6 +250,14 @@ extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *errbuf, in
     if (p->wb < 0) { fail(errbuf, errbuf_len, "partialOrderAlignmentBandConstant must be >= 0 (adaptive band)"); return nullptr; }
     if ((int64_t)p->gap_open1 + p->gap_ext1 >= 65535 || (int64_t)p->gap_open2 + p->gap_ext2 >= 65535) {
         fail(errbuf, errbuf_len, "gap open + extension must be below 65535 (the traceback planes keep E as a 16-bit distance below H)"); return nullptr; }
+    // The sweep's scores are int32, as the reference's are. With every |mat| <= 65535, e <= 65533 < 65534 (from the check above)
+    // and L <= 16383, the largest value it forms, A = H' + (j + 1) e of the F scan, is below 16383 * 65535 + 16384 * 65534 =
+    // 2147368961 < INT32_MAX, and inf_min - min_mis stays above INT32_MIN. Larger scores overflow the reference too (its best
+    // scores then wrap), so there is no answer to reproduce.
+    for (int i = 0; i < 25; ++i)
+        if (p->mat[i] > 65535 || p->mat[i] < -65535) {
+            fail(errbuf, errbuf_len, "partialOrderAlignmentSubMatrix entries must lie in [-65535, 65535] (larger scores overflow the int32 DP "
+                                     "scores, in the reference too)"); return nullptr; }
     if (!p->disable_seeding) { fail(errbuf, errbuf_len, "minimizer seeding (partialOrderAlignmentDisableSeeding=0) is not supported"); return nullptr; }
     if (p->k <= 0 || p->k > 20 || p->w <= 0 || p->w >= 256) { fail(errbuf, errbuf_len, "minimizer k must be in 1..20 and w in 1..255 (guide-tree keys are hash << 24 | span << 16 | read)"); return nullptr; }
     int ndev = 0;

@@ -20,6 +20,7 @@ import _reflib as R  # noqa: E402
 def main():
     assert R.have_ref() and R.have_bar_ref() and R.have_pecan_ref(), "build oracle/_ref first (make -C oracle)"
     rc = pytest.main(["-q", "-p", "no:cacheprovider", os.path.join(ROOT, "tests", "test_oracle_vs_ref.py"),
+                      os.path.join(ROOT, "tests", "test_poa_params_cpu.py"),
                       os.path.join(ROOT, "tests", "test_pecan_cpu.py") + "::test_oracle_vs_reference_random"])
     if rc != 0:
         return int(rc)

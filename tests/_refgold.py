@@ -1,6 +1,6 @@
-"""The unmodified reference's answers for the differential tests (test_oracle_vs_ref.py, test_pecan_cpu.py), stored as SHA-256
-digests in tests/golden/ref_digests.npz so that those tests compare against the reference everywhere, also where the
-reference libraries (oracle/_ref) cannot be built.
+"""The unmodified reference's answers for the differential tests (test_oracle_vs_ref.py, test_poa_params_cpu.py,
+test_pecan_cpu.py), stored as SHA-256 digests in tests/golden/ref_digests.npz so that those tests compare against the reference
+everywhere, also where the reference libraries (oracle/_ref) cannot be built.
 
 Each check has a key (test, case). `check(key, got, ref_fn)` asserts that the digest of `got` equals the stored digest of
 the reference's answer; per-field digests are stored beside it, so that a mismatch names the fields that differ (msa, cigar,
