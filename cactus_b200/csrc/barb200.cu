@@ -9,7 +9,7 @@
 //   * the host does no per-job work besides packing: the guide-tree read orders are computed by the CTA that owns the job
 //     (guide_tree.cuh);
 //   * jobs that outgrow the optimistic plane / MSA sizing come back flagged and are re-run with geometrically larger
-//     slots (x4, then worst case).
+//     slots (x4, then worst case) on the stage's uploaded inputs.
 // A context drives one or more devices; every device has two *lanes* (slot arena + streams + pinned staging) so that one
 // batch's upload / download / unpacking overlaps the other's kernels. host_bar.cpp's dispatcher feeds the lanes of all
 // devices from one queue of ends. No CPU fallback exists: if CUDA is unavailable, creation fails.
@@ -380,52 +380,6 @@ struct Bucket {
     size_t slot_off = 0; int64_t plane_off = 0; size_t clk_off = 0;   // offsets into the lane's arena (bytes / ints / entries)
 };
 
-struct barb200_stage {
-    barb200_ctx *ctx = nullptr;
-    int lane = 0;
-    int64_t n_jobs = 0, n_seqs = 0, n_bases = 0;
-    // everything below is in the stage's INTERNAL job order: class-major (largest class first), cost-descending inside a
-    // class; perm[internal] = the caller's job index
-    std::vector<int64_t> perm;
-    std::vector<int> n_seq, lens, progressive;
-    std::vector<int64_t> soff, job_len_off, job_seq_off, job_sum_len;
-    std::vector<int> job_max_len;
-    std::vector<JobDesc> desc;
-    std::vector<Bucket> buckets;
-    int64_t msa_bytes = 0;
-    double grow = 1.0; bool worst_case = false;
-    // device: one block from the device's cache holds all per-stage arrays
-    void *d_block = nullptr; size_t d_block_bytes = 0;
-    uint8_t *d_seqs = nullptr, *d_msa = nullptr; int *d_lens = nullptr; int64_t *d_soff = nullptr;
-    JobDesc *d_desc = nullptr; int *d_msa_len = nullptr, *d_status = nullptr, *d_next = nullptr; long long *d_cells = nullptr;
-    int *d_order = nullptr, *d_gt_status = nullptr; uint8_t *d_gt_scratch = nullptr;
-    GuideTreeArgs gt; int gt_ctas = 0; float gt_ms = 0.f; cudaEvent_t e_gt = nullptr;   // K0: the guide trees of the stage (guide_tree.cu)
-    // results of the last run
-    std::vector<int> status, msa_len; std::vector<long long> cells;
-    barb200_stage *retry = nullptr; std::vector<int64_t> retry_jobs;     // internal ids
-    int64_t launches = 0; bool ran = false;
-    cudaEvent_t e0 = nullptr, e1 = nullptr; bool launched = false;
-    const uint8_t *host_seqs = nullptr;      // the caller's buffer while it is valid (capacity-miss retries re-upload from it)
-    uint64_t clk[7] = {0, 0, 0, 0, 0, 0, 0};
-};
-
-static void stage_free_device(barb200_stage *st) {
-    dev_free(dev_of_lane(st->ctx, st->lane), st->d_block, st->d_block_bytes);
-    st->d_block = nullptr;
-    st->d_seqs = st->d_msa = nullptr; st->d_lens = nullptr; st->d_soff = nullptr; st->d_desc = nullptr;
-    st->d_msa_len = st->d_status = st->d_next = nullptr; st->d_cells = nullptr; st->d_order = st->d_gt_status = nullptr; st->d_gt_scratch = nullptr;
-}
-
-extern "C" void barb200_stage_destroy(barb200_stage *st) {
-    if (!st) return;
-    cudaSetDevice(dev_of_lane(st->ctx, st->lane).ordinal);
-    if (st->retry) barb200_stage_destroy(st->retry);
-    if (st->e0) { cudaEventDestroy(st->e0); cudaEventDestroy(st->e1); }
-    if (st->e_gt) cudaEventDestroy(st->e_gt);
-    stage_free_device(st);
-    delete st;
-}
-
 static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 static int class_of_len(barb200_ctx *ctx, int64_t max_len) {
@@ -438,6 +392,102 @@ static double job_cost(const barb200_ctx *ctx, int K, int64_t sum, int64_t ml) {
     return (double)(K - 1) * (double)(sum / std::max(1, K) + 1) * std::min<double>((double)ml + 1.0, w) + 2000.0 * K;
 }
 
+// The jobs of one call in the caller's order, scanned and checked once. Stages (and their capacity retries) are lists of indices
+// into it; it keeps its own copy of the lengths because a stage outlives the arguments of barb200_stage_create.
+struct TableJob {
+    int n_seq = 0, max_len = 0, cls = 0, progressive = 0;
+    int64_t len_off = 0, seq_off = 0, sum_len = 0;     // first length in `lens`, first base in the sequence buffer
+    double cost = 0;
+};
+struct JobTable {
+    std::vector<TableJob> jobs;
+    std::vector<int> lens;
+    int64_t n_bases = 0;                                // the sequence buffer: every job's bases back to back
+};
+
+// view(j, len_off, seq_off) -> caller job j, whose lengths and bases the table places at those offsets
+template <class View>
+static int build_table(barb200_ctx *ctx, int64_t n_jobs, View view, JobTable &t) {
+    if (n_jobs > 0x7ffffff0) { set_error(ctx, "too many jobs in one stage"); return BARB200_EINVAL; }
+    t.jobs.resize(n_jobs);
+    int64_t lo = 0, bo = 0;
+    for (int64_t j = 0; j < n_jobs; ++j) {
+        const HostJob v = view(j, lo, bo);
+        if (v.n_seq <= 0) { set_error(ctx, "job without sequences"); return BARB200_EINVAL; }
+        TableJob &J = t.jobs[j];
+        J.n_seq = v.n_seq; J.progressive = v.progressive; J.len_off = lo; J.seq_off = bo;
+        for (int i = 0; i < v.n_seq; ++i) {
+            const int l = v.lens[i];
+            if (l <= 0) { set_error(ctx, "empty sequence in a POA job (the shim substitutes 'N', poaBarAligner.c:551-562)"); return BARB200_EINVAL; }
+            J.sum_len += l; J.max_len = std::max(J.max_len, l);
+        }
+        J.cls = class_of_len(ctx, J.max_len); J.cost = job_cost(ctx, J.n_seq, J.sum_len, J.max_len);
+        if (J.cls < 0) { set_error(ctx, "a sequence is longer than the device engine's row limit (16383 bases per window)"); return BARB200_EINVAL; }
+        if (J.progressive && J.n_seq > 65535) { set_error(ctx, "progressive mode with more than 65535 sequences in one window is not supported"); return BARB200_EINVAL; }
+        t.lens.insert(t.lens.end(), v.lens, v.lens + v.n_seq);
+        lo += v.n_seq; bo += J.sum_len;
+    }
+    t.n_bases = bo;
+    int bad = 0;
+    const int nthreads = host_threads(ctx);
+#pragma omp parallel for schedule(dynamic, 16) num_threads(nthreads) reduction(| : bad)
+    for (int64_t j = 0; j < n_jobs; ++j) {
+        const uint8_t *s = view(j, t.jobs[j].len_off, t.jobs[j].seq_off).seqs;
+        uint8_t m = 0;
+        for (int64_t b = 0; b < t.jobs[j].sum_len; ++b) m |= s[b] > 4;
+        bad |= m;
+    }
+    if (bad) { set_error(ctx, "sequence code > 4"); return BARB200_EINVAL; }
+    return BARB200_OK;
+}
+
+// the jobs as barb200_stage_create and barb200_poa_msa_batch take them: lengths and bases back to back
+static int table_of_arrays(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs, const int *progressive,
+                           JobTable &t) {
+    if (n_jobs < 0 || (n_jobs > 0 && (!n_seq || !seq_lens || !seqs))) { set_error(ctx, "bad arguments"); return BARB200_EINVAL; }
+    return build_table(ctx, n_jobs, [&](int64_t j, int64_t lo, int64_t bo) {
+        return HostJob{n_seq[j], seq_lens + lo, seqs + bo, progressive ? progressive[j] : ctx->hp.progressive_poa};
+    }, t);
+}
+
+static std::vector<int64_t> all_jobs(int64_t n) { std::vector<int64_t> v(n); std::iota(v.begin(), v.end(), (int64_t)0); return v; }
+
+struct barb200_stage {
+    barb200_ctx *ctx = nullptr;
+    int lane = 0;
+    std::shared_ptr<const JobTable> tab;
+    int64_t n_jobs = 0, n_seqs = 0;
+    // everything below is in the stage's INTERNAL job order: class-major (largest class first), cost-descending inside a
+    // class; perm[internal] = the caller's job index in `tab`
+    std::vector<int64_t> perm;
+    std::vector<int> lens;
+    std::vector<int64_t> soff;
+    std::vector<JobDesc> desc;
+    std::vector<Bucket> buckets;
+    int64_t msa_bytes = 0;
+    double grow = 1.0; bool worst_case = false;
+    // device: one block from the device's cache holds all per-stage arrays; a retry's d_seqs are its first stage's
+    void *d_block = nullptr; size_t d_block_bytes = 0;
+    uint8_t *d_seqs = nullptr, *d_msa = nullptr; int *d_lens = nullptr; int64_t *d_soff = nullptr;
+    JobDesc *d_desc = nullptr; int *d_msa_len = nullptr, *d_status = nullptr, *d_next = nullptr; long long *d_cells = nullptr;
+    int *d_order = nullptr, *d_gt_status = nullptr; uint8_t *d_gt_scratch = nullptr;
+    GuideTreeArgs gt; int gt_ctas = 0; cudaEvent_t e_gt = nullptr;   // K0: the guide trees of the stage (guide_tree.cu)
+    std::vector<int> status;                                         // of the last run
+    std::vector<std::unique_ptr<barb200_stage>> retries;             // the last run's capacity retries: x4, then worst case
+    int64_t launches = 0; bool ran = false;
+    cudaEvent_t e0 = nullptr, e1 = nullptr; bool launched = false;
+    uint64_t clk[7] = {0, 0, 0, 0, 0, 0, 0};
+    ~barb200_stage() {
+        cudaSetDevice(dev_of_lane(ctx, lane).ordinal);
+        retries.clear();
+        if (e0) { cudaEventDestroy(e0); cudaEventDestroy(e1); }
+        if (e_gt) cudaEventDestroy(e_gt);
+        dev_free(dev_of_lane(ctx, lane), d_block, d_block_bytes);
+    }
+};
+
+extern "C" void barb200_stage_destroy(barb200_stage *st) { delete st; }
+
 // Slot sizes, shared memory and resident CTAs of every bucket; carve the lane's arena.
 static int plan_stage(barb200_stage *st) {
     barb200_ctx *ctx = st->ctx;
@@ -446,7 +496,8 @@ static int plan_stage(barb200_stage *st) {
     for (Bucket &B : st->buckets) {
         int64_t max_nodes = 4, max_edges = 4, max_len = 1, max_k = 1, plane_need = 0;
         for (int64_t j = B.job_base; j < B.job_base + B.n_jobs; ++j) {
-            const int64_t sum = st->job_sum_len[j], ml = st->job_max_len[j], K = st->n_seq[j];
+            const TableJob &J = st->tab->jobs[st->perm[j]];
+            const int64_t sum = J.sum_len, ml = J.max_len, K = J.n_seq;
             max_nodes = std::max(max_nodes, sum + 2); max_edges = std::max(max_edges, sum + K); max_len = std::max(max_len, ml);
             max_k = std::max(max_k, K);
             plane_need = std::max(plane_need, plane_ints_for_job(ctx->P.wb, ctx->P.wf, K, sum, ml, st->grow, st->worst_case));
@@ -549,89 +600,46 @@ static int ensure_arena(barb200_ctx *ctx, Device &D, Lane &LN, size_t slots_byte
     return BARB200_OK;
 }
 
-// n_seq / seq_lens / seqs / progressive are in the CALLER's job order; seq_off[j] (may be null = consecutive) is the offset of
-// job j's first base in `seqs`, n_bases_total the size of `seqs`. grow / worst_case size the slots (capacity-miss retries).
 static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 static bool timing_on() { static const bool on = getenv("BARB200_TIMING") != nullptr; return on; }
 
-static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs, const int64_t *seq_off,
-                       int64_t n_bases_total, const int *progressive, double grow, bool worst_case, barb200_stage **out) {
-    if (!ctx || n_jobs < 0 || (n_jobs > 0 && (!n_seq || !seq_lens || !seqs))) { set_error(ctx, "bad arguments"); return BARB200_EINVAL; }
-    if (n_jobs > 0x7ffffff0) { set_error(ctx, "too many jobs in one stage"); return BARB200_EINVAL; }
+// A stage over the table's jobs `jobs` (caller indices); grow / worst_case size the slots (capacity-miss retries). A call's first
+// stage uploads the table's bases from `seqs`; a retry runs on its first stage's device copy `d_seqs` and uploads none.
+static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTable> tab, std::vector<int64_t> jobs, double grow, bool worst_case,
+                       const uint8_t *seqs, uint8_t *d_seqs, barb200_stage **out) {
     Device &D = dev_of_lane(ctx, lane);
     Lane &LN = lane_of(ctx, lane);
     cudaSetDevice(D.ordinal);
     std::unique_ptr<barb200_stage> st(new barb200_stage());
-    st->ctx = ctx; st->lane = lane; st->n_jobs = n_jobs; st->grow = grow; st->worst_case = worst_case;
+    const JobTable &T = *tab;
+    const int64_t n_jobs = (int64_t)jobs.size();
+    st->ctx = ctx; st->lane = lane; st->tab = std::move(tab); st->n_jobs = n_jobs; st->grow = grow; st->worst_case = worst_case;
     const double tb0 = now_ms();
-    // ---- caller-order facts ----
-    std::vector<int64_t> c_len_off(n_jobs + 1), c_seq_off(n_jobs + 1), c_sum(n_jobs);
-    std::vector<int> c_ml(n_jobs), c_cls(n_jobs);
-    std::vector<double> c_cost(n_jobs);
-    int64_t ns = 0, nb = 0;
-    for (int64_t j = 0; j < n_jobs; ++j) {
-        if (n_seq[j] <= 0) { set_error(ctx, "job without sequences"); return BARB200_EINVAL; }
-        c_len_off[j] = ns; c_seq_off[j] = seq_off ? seq_off[j] : nb;
-        int64_t sum = 0; int ml = 0;
-        for (int i = 0; i < n_seq[j]; ++i) {
-            const int l = seq_lens[ns + i];
-            if (l <= 0) { set_error(ctx, "empty sequence in a POA job (the shim substitutes 'N', poaBarAligner.c:551-562)"); return BARB200_EINVAL; }
-            sum += l; ml = std::max(ml, l);
-        }
-        c_sum[j] = sum; c_ml[j] = ml; c_cls[j] = class_of_len(ctx, ml); c_cost[j] = job_cost(ctx, n_seq[j], sum, ml);
-        if (c_cls[j] < 0) { set_error(ctx, "a sequence is longer than the device engine's row limit (16383 bases per window)"); return BARB200_EINVAL; }
-        ns += n_seq[j]; nb += sum;
-    }
-    c_len_off[n_jobs] = ns; c_seq_off[n_jobs] = nb;
-    if (!seq_off) n_bases_total = nb;
-    st->n_seqs = ns; st->n_bases = n_bases_total;
-    // input validation (codes 0..4)
-    {
-        int bad = 0;
-        const int nthreads = host_threads(ctx);
-#pragma omp parallel for schedule(static) num_threads(nthreads) reduction(| : bad)
-        for (int64_t b = 0; b < (n_bases_total + 65535) / 65536; ++b) {
-            const int64_t e = std::min<int64_t>(n_bases_total, (b + 1) * 65536);
-            uint8_t m = 0;
-            for (int64_t t = b * 65536; t < e; ++t) m |= seqs[t] > 4;
-            bad |= m;
-        }
-        if (bad) { set_error(ctx, "sequence code > 4"); return BARB200_EINVAL; }
-    }
-    const double tb1 = now_ms();
     // ---- internal order: largest class first, inside a class by estimated cost, largest first (stable) ----
-    st->perm.resize(n_jobs);
-    std::iota(st->perm.begin(), st->perm.end(), (int64_t)0);
+    st->perm = std::move(jobs);
     std::stable_sort(st->perm.begin(), st->perm.end(), [&](int64_t a, int64_t b) {
-        if (c_cls[a] != c_cls[b]) return c_cls[a] > c_cls[b];
-        return c_cost[a] > c_cost[b];
+        if (T.jobs[a].cls != T.jobs[b].cls) return T.jobs[a].cls > T.jobs[b].cls;
+        return T.jobs[a].cost > T.jobs[b].cost;
     });
-    st->n_seq.resize(n_jobs); st->progressive.resize(n_jobs);
-    st->job_len_off.resize(n_jobs + 1); st->job_seq_off.resize(n_jobs + 1); st->job_sum_len.resize(n_jobs); st->job_max_len.resize(n_jobs);
-    st->lens.resize(ns); st->soff.resize(ns); st->desc.resize(n_jobs);
+    st->desc.resize(n_jobs);
     int64_t lo = 0, msa_off = 0;
     for (int64_t j = 0; j < n_jobs; ++j) {
-        const int64_t c = st->perm[j];
-        const int K = n_seq[c];
-        st->n_seq[j] = K; st->progressive[j] = progressive ? progressive[c] : ctx->hp.progressive_poa;
-        st->job_len_off[j] = lo; st->job_seq_off[j] = c_seq_off[c]; st->job_sum_len[j] = c_sum[c]; st->job_max_len[j] = c_ml[c];
+        const TableJob &J = T.jobs[st->perm[j]];
+        const int K = J.n_seq;
         int64_t o = 0;
-        for (int i = 0; i < K; ++i) { st->lens[lo + i] = seq_lens[c_len_off[c] + i]; st->soff[lo + i] = o; o += st->lens[lo + i]; }
-        const int64_t sum = c_sum[c], ml = c_ml[c];
-        int64_t stride = sum;
-        if (!worst_case) stride = std::min<int64_t>(sum, (int64_t)(grow * (double)(ml + ml / 2 + 64)));
+        for (int i = 0; i < K; ++i) { st->lens.push_back(T.lens[J.len_off + i]); st->soff.push_back(o); o += T.lens[J.len_off + i]; }
+        int64_t stride = J.sum_len;
+        if (!worst_case) stride = std::min<int64_t>(J.sum_len, (int64_t)(grow * (double)(J.max_len + J.max_len / 2 + 64)));
         stride = align_up(stride, 16);
         JobDesc &d = st->desc[j];
-        d.n_seq = K; d.seq_off = c_seq_off[c]; d.len_off = lo; d.msa_off = msa_off; d.msa_stride = (int)stride; d.progressive = st->progressive[j];
-        if (d.progressive && K > 65535) { set_error(ctx, "progressive mode with more than 65535 sequences in one window is not supported"); return BARB200_EINVAL; }
+        d.n_seq = K; d.seq_off = J.seq_off; d.len_off = lo; d.msa_off = msa_off; d.msa_stride = (int)stride; d.progressive = J.progressive;
         msa_off += stride * K;
         lo += K;
-        if (st->buckets.empty() || st->buckets.back().cls != c_cls[c]) { Bucket B; B.cls = c_cls[c]; B.job_base = j; st->buckets.push_back(B); }
+        if (st->buckets.empty() || st->buckets.back().cls != J.cls) { Bucket B; B.cls = J.cls; B.job_base = j; st->buckets.push_back(B); }
         st->buckets.back().n_jobs++;
     }
-    st->job_len_off[n_jobs] = lo; st->job_seq_off[n_jobs] = n_bases_total;
+    const int64_t ns = st->n_seqs = lo;
     st->msa_bytes = msa_off;
-    st->host_seqs = seqs;
     if (n_jobs == 0) { *out = st.release(); return BARB200_OK; }
     // device buffers (one cached block) + upload on the lane's copy stream, so that it overlaps a running kernel
     size_t off = 0;
@@ -642,11 +650,12 @@ static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_
     memset(&GA, 0, sizeof(GA));
     {
         int64_t key_need = 64, gx_need = 8, mk = 1;
-        for (int64_t j = 0; j < n_jobs; ++j) {
-            if (!(st->progressive[j] && st->n_seq[j] > 2)) continue;
-            const int64_t sum = st->job_sum_len[j], worst = 2 * (int64_t)ctx->p.w * sum + st->n_seq[j];
+        for (int64_t c : st->perm) {
+            const TableJob &J = T.jobs[c];
+            if (!(J.progressive && J.n_seq > 2)) continue;
+            const int64_t sum = J.sum_len, worst = 2 * (int64_t)ctx->p.w * sum + J.n_seq;
             key_need = std::max(key_need, worst_case ? worst : std::min<int64_t>(worst, (int64_t)(grow * (double)(sum / 2 + 64))));
-            gx_need = std::max(gx_need, sum); mk = std::max<int64_t>(mk, st->n_seq[j]);
+            gx_need = std::max(gx_need, sum); mk = std::max<int64_t>(mk, J.n_seq);
         }
         int64_t kc = 64; while (kc < key_need) kc <<= 1;            // the sort pads to a power of two
         int64_t o = 0;
@@ -656,7 +665,7 @@ static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_
         GA.slot_bytes = align_up(o, 256);
         st->gt_ctas = (int)std::min<int64_t>(std::min<int64_t>(n_jobs, (int64_t)4 * D.sm_count), std::max<int64_t>(1, ((int64_t)2 << 30) / GA.slot_bytes));
     }
-    const size_t o_seqs = sub(n_bases_total), o_lens = sub(ns * 4), o_soff = sub(ns * 8), o_desc = sub(n_jobs * sizeof(JobDesc)),
+    const size_t o_seqs = d_seqs ? 0 : sub(T.n_bases), o_lens = sub(ns * 4), o_soff = sub(ns * 8), o_desc = sub(n_jobs * sizeof(JobDesc)),
                  o_msa = sub(st->msa_bytes), o_msa_len = sub(n_jobs * 4), o_status = sub(n_jobs * 4), o_cells = sub(n_jobs * 8), o_next = sub(4 * (kNumKernels + 1)),
                  o_order = sub(ns * 4), o_gts = sub(n_jobs * 4), o_gtscr = sub((size_t)GA.slot_bytes * st->gt_ctas);
     st->d_block_bytes = off;
@@ -670,7 +679,7 @@ static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_
         st->d_block = nullptr; return BARB200_ENOMEM;
     }
     uint8_t *blk = (uint8_t *)st->d_block;
-    st->d_seqs = blk + o_seqs; st->d_lens = (int *)(blk + o_lens); st->d_soff = (int64_t *)(blk + o_soff);
+    st->d_seqs = d_seqs ? d_seqs : blk + o_seqs; st->d_lens = (int *)(blk + o_lens); st->d_soff = (int64_t *)(blk + o_soff);
     st->d_desc = (JobDesc *)(blk + o_desc); st->d_msa = blk + o_msa; st->d_msa_len = (int *)(blk + o_msa_len); st->d_status = (int *)(blk + o_status);
     st->d_cells = (long long *)(blk + o_cells); st->d_next = (int *)(blk + o_next);
     st->d_order = (int *)(blk + o_order); st->d_gt_status = (int *)(blk + o_gts); st->d_gt_scratch = blk + o_gtscr;
@@ -678,15 +687,15 @@ static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_
     GA.next_job = st->d_next + kNumKernels; GA.scratch = st->d_gt_scratch; GA.k = ctx->p.k; GA.w = ctx->p.w;
     cudaStream_t s = LN.copy;
     const double tb4 = now_ms();
-    if ((e = cudaMemcpyAsync(st->d_seqs, seqs, n_bases_total, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
+    if ((!d_seqs && (e = cudaMemcpyAsync(st->d_seqs, seqs, T.n_bases, cudaMemcpyHostToDevice, s)) != cudaSuccess) ||
         (e = cudaMemcpyAsync(st->d_lens, st->lens.data(), ns * 4, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaMemcpyAsync(st->d_soff, st->soff.data(), ns * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaMemcpyAsync(st->d_desc, st->desc.data(), n_jobs * sizeof(JobDesc), cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaStreamSynchronize(s)) != cudaSuccess) {
-        set_error(ctx, std::string("H2D failed: ") + cudaGetErrorString(e)); stage_free_device(st.get()); return BARB200_ECUDA;
+        set_error(ctx, std::string("H2D failed: ") + cudaGetErrorString(e)); return BARB200_ECUDA;
     }
-    if (timing_on()) fprintf(stderr, "barb200 timing: stage_build: scan + validate %.2f ms, order + descriptors %.2f, plan %.2f, alloc %.2f, upload %.2f\n",
-                             tb1 - tb0, tb2 - tb1, tb3 - tb2, tb4 - tb3, now_ms() - tb4);
+    if (timing_on()) fprintf(stderr, "barb200 timing: stage_build: order + descriptors %.2f ms, plan %.2f, alloc %.2f, upload %.2f\n",
+                             tb2 - tb0, tb3 - tb2, tb4 - tb3, now_ms() - tb4);
     *out = st.release();
     return BARB200_OK;
 }
@@ -694,13 +703,12 @@ static int stage_build(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_
 extern "C" int barb200_stage_create(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens,
                                     const uint8_t *seqs, const int *progressive, barb200_stage **out) {
     if (!ctx || !out) return BARB200_EINVAL;
+    auto tab = std::make_shared<JobTable>();
+    const int rc = table_of_arrays(ctx, n_jobs, n_seq, seq_lens, seqs, progressive, *tab);
+    if (rc) return rc;
     std::lock_guard<std::mutex> lk(lane_of(ctx, 0).busy);
-    int rc = stage_build(ctx, 0, n_jobs, n_seq, seq_lens, seqs, nullptr, 0, progressive, 1.0, false, out);
-    if (!rc) (*out)->host_seqs = nullptr;       // the caller's buffer is only guaranteed during this call
-    return rc;
+    return stage_build(ctx, 0, tab, all_jobs(n_jobs), 1.0, false, seqs, nullptr, out);
 }
-
-static int stage_run_locked(barb200_stage *st, float *kernel_ms);
 
 // queue the stage's kernels on its lane's streams; returns without waiting
 static int stage_launch(barb200_stage *st) {
@@ -710,7 +718,7 @@ static int stage_launch(barb200_stage *st) {
     cudaSetDevice(D.ordinal);
     st->launches = 0; st->ran = false; st->launched = false;
     if (st->n_jobs == 0) return BARB200_OK;
-    if (st->retry) { barb200_stage_destroy(st->retry); st->retry = nullptr; st->retry_jobs.clear(); }
+    st->retries.clear();
     size_t slots_bytes = 0, plane_ints = 0, clk_n = 0;
     for (const Bucket &B : st->buckets) { slots_bytes += (size_t)B.lay.slot_bytes * B.slots; plane_ints += (size_t)B.lay.plane_cap * B.slots; clk_n += (size_t)B.slots * PH_N; }
     if (!ctx->p.collect_phase_clocks) clk_n = 0;
@@ -755,7 +763,8 @@ static int stage_launch(barb200_stage *st) {
     return BARB200_OK;
 }
 
-// wait for the stage's kernels, collect their device time, re-run capacity misses with larger slots
+// wait for the stage's kernels and collect their device time; re-run the capacity misses of each round with larger slots (x4,
+// then worst case) on the stage's uploaded inputs
 static int stage_finish(barb200_stage *st, float *kernel_ms) {
     barb200_ctx *ctx = st->ctx;
     Device &D = dev_of_lane(ctx, st->lane);
@@ -765,80 +774,62 @@ static int stage_finish(barb200_stage *st, float *kernel_ms) {
     if (!st->launched) { set_error(ctx, "stage_finish without stage_launch"); return BARB200_EINVAL; }
     cudaSetDevice(D.ordinal);
     cudaStream_t s = LN.main;
-    cudaError_t se = cudaStreamSynchronize(s);
-    if (se != cudaSuccess) { set_error(ctx, std::string("kernel execution: ") + cudaGetErrorString(se)); return BARB200_ECUDA; }
-    float ms = 0.f; cudaEventElapsedTime(&ms, st->e0, st->e1);
-    st->gt_ms = 0.f; cudaEventElapsedTime(&st->gt_ms, st->e0, st->e_gt);
-    st->launched = false;
-    st->status.resize(st->n_jobs);
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->status.data(), st->d_status, st->n_jobs * 4, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    float ms = 0.f;
     for (int k = 0; k < 7; ++k) st->clk[k] = 0;
-    st->clk[6] = (uint64_t)(st->gt_ms * 1e6f);          // K0 is a kernel of its own: its device time, in nanoseconds
-    if (ctx->p.collect_phase_clocks) {
-        size_t clk_n = 0;
-        for (const Bucket &B : st->buckets) clk_n += (size_t)B.slots * PH_N;
-        std::vector<unsigned long long> h(clk_n);
-        CUDA_TRY(ctx, cudaMemcpy(h.data(), LN.d_clk, clk_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        for (size_t b = 0; b < clk_n / PH_N; ++b) for (int k = 0; k < 6; ++k) st->clk[k] += h[b * PH_N + k];
-    }
-    // capacity misses -> retry launch for just those jobs with larger slots (x4 first, then worst case)
-    std::vector<int64_t> redo;
-    for (int64_t j = 0; j < st->n_jobs; ++j) {
-        const int sc = st->status[j];
-        if (sc == JOB_OK) continue;
-        if (!st->worst_case && (sc == JOB_ERR_PLANE_CAP || sc == JOB_ERR_MSA_CAP || sc == JOB_ERR_GT_CAP)) redo.push_back(j);
-        else {
-            char buf[200];
-            if (sc == JOB_ERR_PLANE_CAP)
-                snprintf(buf, sizeof(buf), "job %lld needs more DP-plane memory than this lane can plan (%.1f GB of planes per slot)", (long long)st->perm[j],
-                         st->buckets.empty() ? 0.0 : (double)st->buckets[0].lay.plane_cap * 4.0 / 1e9);
-            else
-                snprintf(buf, sizeof(buf), "job %lld failed on the device with status %d", (long long)st->perm[j], sc);
-            set_error(ctx, buf); return BARB200_EJOB;
+    for (barb200_stage *r = st;;) {
+        cudaError_t se = cudaStreamSynchronize(s);
+        if (se != cudaSuccess) { set_error(ctx, std::string("kernel execution: ") + cudaGetErrorString(se)); return BARB200_ECUDA; }
+        float rms = 0.f; cudaEventElapsedTime(&rms, r->e0, r->e1);
+        float gt_ms = 0.f; cudaEventElapsedTime(&gt_ms, r->e0, r->e_gt);
+        ms += rms;
+        r->launched = false;
+        r->status.resize(r->n_jobs);
+        CUDA_TRY(ctx, cudaMemcpyAsync(r->status.data(), r->d_status, r->n_jobs * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        st->clk[6] += (uint64_t)(gt_ms * 1e6f);          // K0 is a kernel of its own: its device time, in nanoseconds
+        if (ctx->p.collect_phase_clocks) {
+            size_t clk_n = 0;
+            for (const Bucket &B : r->buckets) clk_n += (size_t)B.slots * PH_N;
+            std::vector<unsigned long long> h(clk_n);
+            CUDA_TRY(ctx, cudaMemcpy(h.data(), LN.d_clk, clk_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+            for (size_t b = 0; b < clk_n / PH_N; ++b) for (int k = 0; k < 6; ++k) st->clk[k] += h[b * PH_N + k];
         }
-    }
-    if (!redo.empty()) {
-        std::vector<int> r_nseq, r_lens, r_prog; std::vector<int64_t> r_off;
-        // the retry stage needs host copies of the inputs: use the caller's buffer while it is valid, else fetch them back
-        std::vector<uint8_t> h_seqs;
-        const uint8_t *src = st->host_seqs;
-        if (!src) {
-            h_seqs.resize(st->n_bases);
-            CUDA_TRY(ctx, cudaMemcpy(h_seqs.data(), st->d_seqs, st->n_bases, cudaMemcpyDeviceToHost));
-            src = h_seqs.data();
+        // capacity misses -> retry launch for just those jobs with larger slots (x4 first, then worst case)
+        std::vector<int64_t> redo;
+        for (int64_t j = 0; j < r->n_jobs; ++j) {
+            const int sc = r->status[j];
+            if (sc == JOB_OK) continue;
+            if (!r->worst_case && (sc == JOB_ERR_PLANE_CAP || sc == JOB_ERR_MSA_CAP || sc == JOB_ERR_GT_CAP)) redo.push_back(r->perm[j]);
+            else {
+                char buf[200];
+                if (sc == JOB_ERR_PLANE_CAP)
+                    snprintf(buf, sizeof(buf), "job %lld needs more DP-plane memory than this lane can plan (%.1f GB of planes per slot)", (long long)r->perm[j],
+                             r->buckets.empty() ? 0.0 : (double)r->buckets[0].lay.plane_cap * 4.0 / 1e9);
+                else
+                    snprintf(buf, sizeof(buf), "job %lld failed on the device with status %d", (long long)r->perm[j], sc);
+                set_error(ctx, buf); return BARB200_EJOB;
+            }
         }
-        for (int64_t j : redo) {
-            r_nseq.push_back(st->n_seq[j]); r_prog.push_back(st->progressive[j]); r_off.push_back(st->job_seq_off[j]);
-            for (int i = 0; i < st->n_seq[j]; ++i) r_lens.push_back(st->lens[st->job_len_off[j] + i]);
-        }
+        if (redo.empty()) break;
         barb200_stage *rs = nullptr;
-        const bool go_worst = st->grow >= 4.0;
-        int rc = stage_build(ctx, st->lane, (int64_t)redo.size(), r_nseq.data(), r_lens.data(), src, r_off.data(), st->n_bases, r_prog.data(),
-                             go_worst ? 1.0 : st->grow * 4.0, go_worst, &rs);
+        const bool go_worst = r->grow >= 4.0;
+        int rc = stage_build(ctx, st->lane, st->tab, std::move(redo), go_worst ? 1.0 : r->grow * 4.0, go_worst, nullptr, st->d_seqs, &rs);
         if (rc) return rc;
-        float rms = 0.f;
-        rc = stage_run_locked(rs, &rms);
-        rs->host_seqs = nullptr;
-        if (rc) { barb200_stage_destroy(rs); return rc; }
-        st->retry = rs; st->retry_jobs = redo; st->launches += rs->launches; ms += rms;
-        for (int k = 0; k < 7; ++k) st->clk[k] += rs->clk[k];
+        st->retries.emplace_back(rs);
+        if ((rc = stage_launch(rs))) return rc;
+        st->launches += rs->launches;
+        r = rs;
     }
     if (kernel_ms) *kernel_ms = ms;
     st->ran = true;
     return BARB200_OK;
 }
 
-static int stage_run_locked(barb200_stage *st, float *kernel_ms) {
-    int rc = stage_launch(st);
-    if (rc) return rc;
-    return stage_finish(st, kernel_ms);
-}
-
 extern "C" int barb200_stage_run(barb200_stage *st, float *kernel_ms) {
     if (!st) return BARB200_EINVAL;
     std::lock_guard<std::mutex> lk(lane_of(st->ctx, st->lane).busy);
-    return stage_run_locked(st, kernel_ms);
+    const int rc = stage_launch(st);
+    return rc ? rc : stage_finish(st, kernel_ms);
 }
 
 extern "C" int64_t barb200_stage_launches(barb200_stage *st) { return st ? st->launches : 0; }
@@ -864,50 +855,44 @@ extern "C" int barb200_stage_buckets(barb200_stage *st, int64_t *out, int max_bu
 // dest(caller job index, K, msa_len) -> where the K x msa_len bytes go (nullptr: allocation failure)
 typedef std::function<uint8_t *(int64_t, int, int)> MsaDest;
 
-static int stage_fetch_locked(barb200_stage *st, const MsaDest &dest, int *msa_len, int64_t *cells, const std::vector<int64_t> *outer = nullptr) {
+// every job's result comes from the round that completed it: the stage itself or one of its retries
+static int stage_fetch_locked(barb200_stage *st, const MsaDest &dest, int *msa_len, int64_t *cells) {
     barb200_ctx *ctx = st->ctx;
     Device &D = dev_of_lane(ctx, st->lane);
     Lane &LN = lane_of(ctx, st->lane);
     if (!st->ran) { set_error(ctx, "stage_fetch before stage_run"); return BARB200_EINVAL; }
     if (st->n_jobs == 0) return BARB200_OK;
     cudaSetDevice(D.ordinal);
-    // caller index of internal job j (a retry stage's "caller" is the parent stage: `outer` maps its job list to the real caller)
-    auto caller_of = [&](int64_t j) { const int64_t c = st->perm[j]; return outer ? (*outer)[c] : c; };
-    // the retry stage first: it shares the lane's pinned staging buffer
-    if (st->retry) {
-        std::vector<int64_t> op(st->retry_jobs.size());
-        for (size_t i = 0; i < op.size(); ++i) op[i] = caller_of(st->retry_jobs[i]);
-        int rc = stage_fetch_locked(st->retry, dest, msa_len, cells, &op);
-        if (rc) return rc;
-    }
-    st->msa_len.resize(st->n_jobs); st->cells.resize(st->n_jobs);
-    PinnedBlock down(D, (size_t)st->msa_bytes);
-    if (!down.p) { set_error(ctx, "cudaMallocHost failed"); return BARB200_ENOMEM; }
-    uint8_t *h_msa = (uint8_t *)down.p;
-    cudaStream_t s = LN.main;
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->msa_len.data(), st->d_msa_len, st->n_jobs * 4, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->cells.data(), st->d_cells, st->n_jobs * 8, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(h_msa, st->d_msa, st->msa_bytes, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    std::vector<char> redone(st->n_jobs, 0);
-    for (int64_t j : st->retry_jobs) redone[j] = 1;
-    int oom = 0;
-    const int nthreads = host_threads(ctx);
+    std::vector<barb200_stage *> rounds{st};
+    for (auto &rs : st->retries) rounds.push_back(rs.get());
+    for (barb200_stage *r : rounds) {
+        std::vector<int> r_len(r->n_jobs); std::vector<long long> r_cells(r->n_jobs);
+        PinnedBlock down(D, (size_t)r->msa_bytes);
+        if (!down.p) { set_error(ctx, "cudaMallocHost failed"); return BARB200_ENOMEM; }
+        uint8_t *h_msa = (uint8_t *)down.p;
+        cudaStream_t s = LN.main;
+        CUDA_TRY(ctx, cudaMemcpyAsync(r_len.data(), r->d_msa_len, r->n_jobs * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaMemcpyAsync(r_cells.data(), r->d_cells, r->n_jobs * 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaMemcpyAsync(h_msa, r->d_msa, r->msa_bytes, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        int oom = 0;
+        const int nthreads = host_threads(ctx);
 #pragma omp parallel for schedule(static) num_threads(nthreads) reduction(| : oom)
-    for (int64_t j = 0; j < st->n_jobs; ++j) {
-        if (redone[j]) continue;
-        const int64_t c = caller_of(j);
-        const int K = st->n_seq[j], ml = st->msa_len[j];
-        if (msa_len) msa_len[c] = ml;
-        if (cells) cells[c] = st->cells[j];
-        if (dest) {
-            uint8_t *o = dest(c, K, ml);
-            if (!o) { oom = 1; continue; }
-            const uint8_t *src = h_msa + st->desc[j].msa_off;
-            for (int i = 0; i < K; ++i) memcpy(o + (size_t)i * ml, src + (size_t)i * st->desc[j].msa_stride, ml);
+        for (int64_t j = 0; j < r->n_jobs; ++j) {
+            if (r->status[j] != JOB_OK) continue;           // re-run by a later round
+            const int64_t c = r->perm[j];
+            const int K = r->desc[j].n_seq, ml = r_len[j];
+            if (msa_len) msa_len[c] = ml;
+            if (cells) cells[c] = r_cells[j];
+            if (dest) {
+                uint8_t *o = dest(c, K, ml);
+                if (!o) { oom = 1; continue; }
+                const uint8_t *src = h_msa + r->desc[j].msa_off;
+                for (int i = 0; i < K; ++i) memcpy(o + (size_t)i * ml, src + (size_t)i * r->desc[j].msa_stride, ml);
+            }
         }
+        if (oom) { set_error(ctx, "host allocation failed"); return BARB200_ENOMEM; }
     }
-    if (oom) { set_error(ctx, "host allocation failed"); return BARB200_ENOMEM; }
     return BARB200_OK;
 }
 
@@ -923,12 +908,14 @@ extern "C" int barb200_stage_fetch(barb200_stage *st, uint8_t **msa_out, int *ms
 }
 
 
-// one device batch on one lane (the caller holds the lane): build + launch + streamed guide trees + finish + fetch
-static int batch_on_lane(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs, const int64_t *seq_off,
-                         int64_t n_bases, const int *progressive, const MsaDest &dest, int *msa_len, int64_t *cells, float *device_ms) {
+// one device batch of the table's jobs `jobs` on one lane (the caller holds the lane): build + launch + streamed guide trees +
+// finish + fetch; results land at the caller's job indices
+static int batch_on_lane(barb200_ctx *ctx, int lane, const std::shared_ptr<const JobTable> &tab, std::vector<int64_t> jobs, const uint8_t *seqs,
+                         const MsaDest &dest, int *msa_len, int64_t *cells) {
     barb200_stage *st = nullptr;
+    const int64_t n_jobs = (int64_t)jobs.size();
     const double t0 = now_ms();
-    int rc = stage_build(ctx, lane, n_jobs, n_seq, seq_lens, seqs, seq_off, n_bases, progressive, 1.0, false, &st);
+    int rc = stage_build(ctx, lane, tab, std::move(jobs), 1.0, false, seqs, nullptr, &st);
     if (rc) return rc;
     const double t1 = now_ms(); float kms = 0.f;
     rc = stage_launch(st);
@@ -937,7 +924,6 @@ static int batch_on_lane(barb200_ctx *ctx, int lane, int64_t n_jobs, const int *
     if (!rc) rc = stage_fetch_locked(st, dest, msa_len, cells);
     const double t3 = now_ms();
     barb200_stage_destroy(st);
-    if (device_ms) *device_ms = kms;
     {
         std::lock_guard<std::mutex> lk(ctx->err_mu);
         ctx->last_timing[0] = t1 - t0; ctx->last_timing[1] = t2 - t1; ctx->last_timing[2] = kms; ctx->last_timing[3] = t3 - t2;
@@ -955,36 +941,21 @@ static const int64_t kMaxBasesPerBatch = (int64_t)768 << 20;
 extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens,
                                      const uint8_t *seqs, const int *progressive, uint8_t **msa_out, int *msa_len,
                                      int64_t *cells) {
-    if (!ctx || n_jobs < 0 || (n_jobs > 0 && (!n_seq || !seq_lens || !seqs))) { if (ctx) set_error(ctx, "bad arguments"); return BARB200_EINVAL; }
+    if (!ctx) return BARB200_EINVAL;
     if (msa_out) for (int64_t j = 0; j < n_jobs; ++j) msa_out[j] = nullptr;
-    if (n_jobs == 0) return BARB200_OK;
-    // offsets + estimated cost in the caller's order
-    std::vector<int64_t> len_off(n_jobs + 1), seq_off(n_jobs + 1);
-    std::vector<double> cost(n_jobs);
-    int64_t ns = 0, nb = 0;
-    for (int64_t j = 0; j < n_jobs; ++j) {
-        if (n_seq[j] <= 0) { set_error(ctx, "job without sequences"); return BARB200_EINVAL; }
-        len_off[j] = ns; seq_off[j] = nb;
-        int64_t sum = 0, ml = 0;
-        for (int i = 0; i < n_seq[j]; ++i) {
-            const int l = seq_lens[ns + i];
-            if (l <= 0) { set_error(ctx, "empty sequence in a POA job (the shim substitutes 'N', poaBarAligner.c:551-562)"); return BARB200_EINVAL; }
-            sum += l; ml = std::max<int64_t>(ml, l);
-        }
-        cost[j] = job_cost(ctx, n_seq[j], sum, ml);
-        ns += n_seq[j]; nb += sum;
-    }
-    len_off[n_jobs] = ns; seq_off[n_jobs] = nb;
+    auto tab = std::make_shared<JobTable>();
+    const int trc = table_of_arrays(ctx, n_jobs, n_seq, seq_lens, seqs, progressive, *tab);
+    if (trc || n_jobs == 0) return trc;
+    const std::vector<TableJob> &J = tab->jobs;
     const int ndev = (int)ctx->devs.size();
     // ---- deal: one device -> everything; several -> cost-sorted, each job to the device with the least work so far (LPT, SURVEY.md 8e) ----
     std::vector<std::vector<int64_t>> share(ndev);
-    if (ndev == 1) { share[0].resize(n_jobs); std::iota(share[0].begin(), share[0].end(), (int64_t)0); }
+    if (ndev == 1) share[0] = all_jobs(n_jobs);
     else {
-        std::vector<int64_t> idx(n_jobs);
-        std::iota(idx.begin(), idx.end(), (int64_t)0);
-        std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return cost[a] > cost[b]; });
+        std::vector<int64_t> idx = all_jobs(n_jobs);
+        std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return J[a].cost > J[b].cost; });
         std::vector<double> load(ndev, 0.0);
-        for (int64_t j : idx) { const int d = (int)(std::min_element(load.begin(), load.end()) - load.begin()); share[d].push_back(j); load[d] += cost[j]; }
+        for (int64_t j : idx) { const int d = (int)(std::min_element(load.begin(), load.end()) - load.begin()); share[d].push_back(j); load[d] += J[j].cost; }
         for (auto &s : share) std::sort(s.begin(), s.end());
     }
     std::vector<int> rcs(ndev, BARB200_OK);
@@ -1000,25 +971,11 @@ extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int
         while (at < mine.size() && rcs[d] == BARB200_OK) {
             // one chunk: a bounded number of jobs and bases
             size_t end = at; int64_t bases = 0;
-            while (end < mine.size() && (int64_t)(end - at) < kMaxJobsPerBatch &&
-                   (end == at || bases + (seq_off[mine[end] + 1] - seq_off[mine[end]]) <= kMaxBasesPerBatch)) {
-                bases += seq_off[mine[end] + 1] - seq_off[mine[end]]; ++end;
+            while (end < mine.size() && (int64_t)(end - at) < kMaxJobsPerBatch && (end == at || bases + J[mine[end]].sum_len <= kMaxBasesPerBatch)) {
+                bases += J[mine[end]].sum_len; ++end;
             }
-            const int64_t m = (int64_t)(end - at);
-            std::vector<int> c_nseq(m), c_lens, c_prog(m);
-            std::vector<int64_t> c_off(m);
-            for (int64_t k = 0; k < m; ++k) {
-                const int64_t j = mine[at + k];
-                c_nseq[k] = n_seq[j]; c_prog[k] = progressive ? progressive[j] : ctx->hp.progressive_poa; c_off[k] = seq_off[j];
-                c_lens.insert(c_lens.end(), seq_lens + len_off[j], seq_lens + len_off[j + 1]);
-            }
-            std::vector<int> c_ml(m); std::vector<int64_t> c_cells(m);
-            const int64_t *jobs_of = mine.data() + at;
-            MsaDest dest;
-            if (msa_out) dest = [msa_out, jobs_of](int64_t c, int K, int ml) { uint8_t *o = (uint8_t *)malloc((size_t)K * (ml > 0 ? ml : 1)); msa_out[jobs_of[c]] = o; return o; };
-            const int rc = batch_on_lane(ctx, lane, m, c_nseq.data(), c_lens.data(), seqs, c_off.data(), nb, c_prog.data(), dest, c_ml.data(), c_cells.data(), nullptr);
+            const int rc = batch_on_lane(ctx, lane, tab, std::vector<int64_t>(mine.begin() + at, mine.begin() + end), seqs, malloc_dest(msa_out), msa_len, cells);
             if (rc) { rcs[d] = rc; errs[d] = get_error(ctx); break; }
-            for (int64_t k = 0; k < m; ++k) { if (msa_len) msa_len[jobs_of[k]] = c_ml[k]; if (cells) cells[jobs_of[k]] = c_cells[k]; }
             at = end;
         }
     };
@@ -1035,7 +992,7 @@ extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int
     return BARB200_OK;
 }
 
-// host-side phases of the most recent device batch, milliseconds: out[0] build (pack, validation, planning, H2D), out[1] launch +
+// host-side phases of the most recent device batch, milliseconds: out[0] build (ordering, planning, H2D), out[1] launch +
 // streamed guide trees + wait, out[2] device time of the kernels, out[3] fetch (D2H + unpack), out[4] total, out[5] jobs
 extern "C" int barb200_last_batch_timing(barb200_ctx *ctx, double out[6]) {
     if (!ctx || !out) return BARB200_EINVAL;
@@ -1051,27 +1008,24 @@ int run_jobs_on_lane(barb200_ctx *ctx, int lane, const std::vector<HostJob> &job
     const int64_t n = (int64_t)jobs.size();
     results.assign(n, JobResult());
     if (n == 0) return BARB200_OK;
+    auto tab = std::make_shared<JobTable>();
+    int rc = build_table(ctx, n, [&](int64_t j, int64_t, int64_t) { return jobs[j]; }, *tab);
+    if (rc) return rc;
+    const std::vector<TableJob> &J = tab->jobs;
     Lane &LN = lane_of(ctx, lane);
     std::lock_guard<std::mutex> lk(LN.busy);
     cudaSetDevice(dev_of_lane(ctx, lane).ordinal);
-    std::vector<int> n_seq(n), prog(n), lens; std::vector<int64_t> off(n + 1);
-    int64_t nb = 0;
-    for (int64_t j = 0; j < n; ++j) {
-        n_seq[j] = jobs[j].n_seq; prog[j] = jobs[j].progressive; off[j] = nb;
-        for (int i = 0; i < jobs[j].n_seq; ++i) { lens.push_back(jobs[j].lens[i]); nb += jobs[j].lens[i]; }
-    }
-    off[n] = nb;
-    PinnedBlock up(dev_of_lane(ctx, lane), (size_t)nb);
+    PinnedBlock up(dev_of_lane(ctx, lane), (size_t)tab->n_bases);
     if (!up.p) { set_error(ctx, "cudaMallocHost failed"); return BARB200_ENOMEM; }
     uint8_t *const h_up = (uint8_t *)up.p;
     const int nthreads = host_threads(ctx);
 #pragma omp parallel for schedule(static) num_threads(nthreads)
-    for (int64_t j = 0; j < n; ++j) memcpy(h_up + off[j], jobs[j].seqs, (size_t)(off[j + 1] - off[j]));
+    for (int64_t j = 0; j < n; ++j) memcpy(h_up + J[j].seq_off, jobs[j].seqs, (size_t)J[j].sum_len);
     std::vector<int> ml(n, 0); std::vector<int64_t> cells(n, 0);
     JobResult *res = results.data();
     static uint8_t empty_sink[1];
     MsaDest dest = [res](int64_t c, int K, int m) { res[c].msa.resize((size_t)K * m); return res[c].msa.empty() ? empty_sink : res[c].msa.data(); };
-    const int rc = batch_on_lane(ctx, lane, n, n_seq.data(), lens.data(), h_up, nullptr, nb, prog.data(), dest, ml.data(), cells.data(), nullptr);
+    rc = batch_on_lane(ctx, lane, tab, all_jobs(n), h_up, dest, ml.data(), cells.data());
     if (rc) return rc;
     for (int64_t j = 0; j < n; ++j) { results[j].msa_len = ml[j]; results[j].cells = cells[j]; }
     return BARB200_OK;

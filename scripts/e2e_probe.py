@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Development aid: time barb200_poa_msa_batch (host buffers) on the bench shape, pipelined vs single stage."""
+"""Development aid: time barb200_poa_msa_batch (host buffers) on the bench shape (argument: number of ends)."""
 import os, sys, time
 import numpy as np
 import ctypes as C

@@ -194,27 +194,33 @@ def test_windows_vs_oracle_and_invariant(engine, oracle_built):
 
 
 def test_errors_are_loud(engine):
+    """every rejection of the job checks raises through both the batch call and the stage; the progressive job of 65536 reads is
+    refused on the host before any device work"""
     import cactus_b200 as cb
-    with pytest.raises(cb.BarB200Error):
-        engine.poa_msa_batch([[np.array([0, 1, 7], np.uint8), np.array([0, 1], np.uint8)]])
-    with pytest.raises(cb.BarB200Error):
-        engine.poa_msa_batch([[np.array([], np.uint8), np.array([0, 1], np.uint8)]])
-    with pytest.raises(cb.BarB200Error):            # one base past the largest CTA class (1024 threads x 16 columns - 1)
-        engine.poa_msa_batch([[np.zeros(16384, np.uint8), np.array([0, 1], np.uint8)]])
+    ok = np.array([0, 1], np.uint8)
+    bad = [([[ok], []], "job without sequences"),
+           ([[np.array([], np.uint8), ok]], "empty sequence"),
+           ([[np.array([0, 1, 7], np.uint8), ok]], "sequence code > 4"),
+           ([[np.zeros(16384, np.uint8), ok]], "row limit"),         # one base past the largest CTA class (1024 threads x 16 columns - 1)
+           ([[np.zeros(1, np.uint8)] * 65536], "more than 65535 sequences")]
+    for jobs, msg in bad:
+        for submit in (engine.poa_msa_batch, engine.stage):
+            with pytest.raises(cb.BarB200Error, match=msg):
+                submit(jobs)
     with pytest.raises(cb.BarB200Error):
         cb.Engine(cb.PoaParams(partialOrderAlignmentGapOpenPenalty2=0))
 
 
-def test_pipelined_batch_equals_single_stage(engine, oracle_built):
-    """a batch large enough to be cut into pipelined chunks (producer thread, two slot arenas, two streams) returns
-    exactly what one single-stage launch returns; spot-checked against the oracle"""
+def test_chunked_batch_equals_single_stage(engine, oracle_built):
+    """a batch of more jobs than one device batch takes (1 << 15) is cut into chunks and returns exactly what one stage over
+    every job returns; spot-checked against the oracle in both chunks"""
     rng = np.random.default_rng(46)
     jobs = []
-    for it in range(2600):
+    for it in range(40000):
         K = int(rng.integers(2, 6))
         L = int(rng.choice([8, 30, 70, 120]))
         jobs.append(family(rng, K, L, sub=0.05, ins=0.02, dele=0.02))
-    msas, cells = engine.poa_msa_batch(jobs, return_cells=True)          # pipelined path (>= 2 * 8 * SMs jobs)
+    msas, cells = engine.poa_msa_batch(jobs, return_cells=True)
     st = engine.stage(jobs)
     st.run()
     msas1, cells1 = st.fetch()
@@ -248,12 +254,16 @@ def test_mixed_shapes_are_bucketed(engine, oracle_built):
     assert b[0]["plane_ints"] > 20 * b[-1]["plane_ints"]          # slots are sized per class, not from the largest job
 
 
-def test_capacity_misses_grow_geometrically(oracle_built):
-    """unrelated sequences outgrow the optimistic plane / MSA sizing: the flagged jobs are re-run with x4 slots, then at worst
-    case, and still equal the oracle"""
+def _capacity_miss_jobs():
+    """unrelated sequences, which outgrow the optimistic plane / MSA sizing, and related families, which do not"""
     rng = np.random.default_rng(48)
     jobs = [[rng.integers(0, 4, size=int(rng.integers(150, 400))).astype(np.uint8) for _ in range(int(rng.integers(6, 12)))] for _ in range(10)]
-    jobs += [family(rng, 4, 300) for _ in range(6)]
+    return jobs + [family(rng, 4, 300) for _ in range(6)]
+
+
+def test_capacity_misses_grow_geometrically(oracle_built):
+    """the flagged jobs are re-run with x4 slots, then at worst case, and still equal the oracle"""
+    jobs = _capacity_miss_jobs()
     import cactus_b200 as cb
     e = cb.Engine()
     msas = e.poa_msa_batch(jobs)
@@ -261,6 +271,27 @@ def test_capacity_misses_grow_geometrically(oracle_built):
     for j, job in enumerate(jobs):
         o = R.oracle_poa_msa(job)
         assert msas[j].shape == o.shape and np.array_equal(msas[j], o), j
+
+
+def test_capacity_misses_retried_by_a_stage(oracle_built):
+    """the same jobs through a stage, which keeps its inputs on the device: every run re-runs the flagged jobs there (more launches
+    than the first round's guide-tree kernel and one launch per bucket), and fetch returns what the batch call and the oracle return"""
+    jobs = _capacity_miss_jobs()
+    import cactus_b200 as cb
+    e = cb.Engine()
+    msas, cells = e.poa_msa_batch(jobs, return_cells=True)
+    st = e.stage(jobs)
+    for _ in range(2):
+        st.run()
+        assert st.launches() > 1 + len(st.buckets())
+    smsas, scells = st.fetch()
+    st.close()
+    e.close()
+    assert np.array_equal(np.asarray(scells), np.asarray(cells))
+    for j, job in enumerate(jobs):
+        tr = R.oracle_poa_msa_trace(job)
+        assert smsas[j].shape == tr["msa"].shape and np.array_equal(smsas[j], tr["msa"]), j
+        assert np.array_equal(msas[j], smsas[j]) and int(scells[j]) == tr["cells"], j
 
 
 def test_band_wider_than_planned_is_retried(oracle_built):
