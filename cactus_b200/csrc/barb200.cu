@@ -29,7 +29,6 @@
 #include <string>
 #include <vector>
 #include "host_api.h"
-#include "batch_merge.h"
 #include "poa_kernel.cuh"
 #include "slot_plan.h"
 
@@ -81,12 +80,9 @@ struct barb200_ctx {
     std::vector<std::unique_ptr<Device>> devs;
     int lanes_per_device = 2;
     bool lanes_shared = false;          // set once the dispatcher runs: every lane plans with its share of the device memory
-    std::mutex mu;                      // serialises the pair-HMM batches (device 0)
     std::mutex err_mu;
     std::string err;
-    GroupCommit<PecanRequest> pecan_group;  // concurrent barb200_pecan_aligned_pairs_batch callers share device batches
-    void *pecan_scratch = nullptr; size_t pecan_scratch_bytes = 0;   // pecan.cu's batch call (grow-only)
-    void *pecan_pinned[2] = {nullptr, nullptr}; size_t pecan_pinned_bytes[2] = {0, 0};   // pinned staging: 0 upload, 1 download
+    void *pecan = nullptr;              // pecan.cu's pair-HMM state (created and destroyed with the context)
     void *dispatcher = nullptr;         // host_bar.cpp's end queue (created on first use, destroyed with the context)
     double last_timing[6] = {0, 0, 0, 0, 0, 0};   // of the most recent device batch (barb200_last_batch_timing), under err_mu
 };
@@ -129,12 +125,12 @@ int host_threads(barb200_ctx *ctx) {
     return std::max(1, n / std::max(1, tl_thread_divisor));
 }
 int default_progressive(barb200_ctx *ctx) { return ctx->p.progressive_poa; }
-std::mutex &device_mutex(barb200_ctx *ctx) { return ctx->mu; }
 int ctx_device(barb200_ctx *ctx) { return ctx->devs[0]->ordinal; }
 int ctx_sm_count(barb200_ctx *ctx) { return ctx->devs[0]->sm_count; }
 double ctx_mem_fraction(barb200_ctx *ctx) { return ctx->p.mem_fraction > 0 ? ctx->p.mem_fraction : 0.85; }
 int total_lanes(barb200_ctx *ctx) { return (int)ctx->devs.size() * ctx->lanes_per_device; }
 void **dispatcher_slot(barb200_ctx *ctx) { return &ctx->dispatcher; }
+void **pecan_slot(barb200_ctx *ctx) { return &ctx->pecan; }
 void mark_lanes_shared(barb200_ctx *ctx) { ctx->lanes_shared = true; }
 static Device &dev_of_lane(barb200_ctx *ctx, int lane) { return *ctx->devs[lane / ctx->lanes_per_device]; }
 static Lane &lane_of(barb200_ctx *ctx, int lane) { return *ctx->devs[lane / ctx->lanes_per_device]->lanes[lane % ctx->lanes_per_device]; }
@@ -203,30 +199,9 @@ static void dev_free(Device &D, void *p, size_t bytes) {
 namespace barb200 {
 int device_alloc(barb200_ctx *ctx, void **p, size_t bytes) { return dev_alloc(*ctx->devs[0], p, bytes) == cudaSuccess ? 0 : -1; }
 void device_free(barb200_ctx *ctx, void *p, size_t bytes) { dev_free(*ctx->devs[0], p, bytes); }
-// grow-only scratch of the pair-HMM batch call (tens of GB of rings: cudaMalloc of that size costs ~0.2 s per call)
-void *pecan_scratch(barb200_ctx *ctx, size_t bytes) {
-    if (ctx->pecan_scratch_bytes >= bytes && ctx->pecan_scratch) return ctx->pecan_scratch;
-    if (ctx->pecan_scratch) { cudaFree(ctx->pecan_scratch); ctx->pecan_scratch = nullptr; ctx->pecan_scratch_bytes = 0; }
-    void *p = nullptr;
-    if (cudaMalloc(&p, bytes) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    ctx->pecan_scratch = p; ctx->pecan_scratch_bytes = bytes;
-    return p;
-}
-// grow-only pinned staging buffers of the pair-HMM batch call (which: 0 upload, 1 download); nullptr on failure
-void *pecan_pinned(barb200_ctx *ctx, int which, size_t bytes) {
-    if (ctx->pecan_pinned_bytes[which] >= bytes && ctx->pecan_pinned[which]) return ctx->pecan_pinned[which];
-    if (ctx->pecan_pinned[which]) { cudaFreeHost(ctx->pecan_pinned[which]); ctx->pecan_pinned[which] = nullptr; ctx->pecan_pinned_bytes[which] = 0; }
-    void *p = nullptr;
-    bytes += bytes / 4;
-    if (cudaMallocHost(&p, bytes) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    ctx->pecan_pinned[which] = p; ctx->pecan_pinned_bytes[which] = bytes;
-    return p;
-}
-GroupCommit<PecanRequest> &pecan_group(barb200_ctx *ctx) { return ctx->pecan_group; }
+void *pinned_take(barb200_ctx *ctx, size_t bytes, size_t *got) { return ::pinned_take(*ctx->devs[0], bytes, got); }
+void pinned_give(barb200_ctx *ctx, void *p, size_t bytes) { ::pinned_give(*ctx->devs[0], p, bytes); }
 }  // namespace barb200
-
-#define CUDA_TRY(ctx, call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { \
-    set_error(ctx, std::string(#call) + ": " + cudaGetErrorString(_e)); return BARB200_ECUDA; } } while (0)
 
 extern "C" void barb200_params_default(barb200_params *p) {
     static const int mat[25] = {91, -114, -61, -123, -100, -114, 100, -125, -61, -100, -61, -125, 100, -114, -100,
@@ -306,10 +281,9 @@ extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *errbuf, in
         if (!ok) { fail(errbuf, errbuf_len, "creating streams / pinned memory failed"); barb200_destroy(ctx.release()); return nullptr; }
     }
     cudaSetDevice(ords[0]);
+    if (pecan_create(ctx.get()) != 0) { fail(errbuf, errbuf_len, "creating streams / pinned memory failed"); barb200_destroy(ctx.release()); return nullptr; }
     return ctx.release();
 }
-
-namespace barb200 { void dispatcher_destroy(barb200_ctx *ctx); }
 
 extern "C" void barb200_destroy(barb200_ctx *ctx) {
     if (!ctx) return;
@@ -328,8 +302,7 @@ extern "C" void barb200_destroy(barb200_ctx *ctx) {
         for (auto &b : D->free_pinned) cudaFreeHost(b.first);
     }
     if (!ctx->devs.empty()) cudaSetDevice(ctx->devs[0]->ordinal);
-    if (ctx->pecan_scratch) cudaFree(ctx->pecan_scratch);
-    for (int i = 0; i < 2; ++i) if (ctx->pecan_pinned[i]) cudaFreeHost(ctx->pecan_pinned[i]);
+    pecan_destroy(ctx);
     delete ctx;
 }
 

@@ -1,7 +1,6 @@
 // host_api.h -- internal C++ interfaces between the host-side translation units of libbarb200.
 #pragma once
 #include <stdint.h>
-#include <mutex>
 #include <string>
 #include <vector>
 #include "../../include/barb200.h"
@@ -37,15 +36,23 @@ void set_error(barb200_ctx *ctx, const std::string &msg);
 std::string get_error(barb200_ctx *ctx);
 int host_threads(barb200_ctx *ctx);
 int default_progressive(barb200_ctx *ctx);
-// context facts for the other translation units (pecan.cu)
-std::mutex &device_mutex(barb200_ctx *ctx);    // serialises the pair-HMM batches on one context
+// context facts for pecan.cu, which runs the pair-HMM work on the context's first device
 int ctx_device(barb200_ctx *ctx);
 int ctx_sm_count(barb200_ctx *ctx);
 double ctx_mem_fraction(barb200_ctx *ctx);
-// device blocks from the context's grow-only cache (cudaMalloc / cudaFree per call cost milliseconds); 0 on success
+// device blocks from the first device's grow-only cache (cudaMalloc / cudaFree per call cost milliseconds); 0 on success
 int device_alloc(barb200_ctx *ctx, void **p, size_t bytes);
 void device_free(barb200_ctx *ctx, void *p, size_t bytes);
-void *pecan_scratch(barb200_ctx *ctx, size_t bytes);
-void *pecan_pinned(barb200_ctx *ctx, int which, size_t bytes);   // grow-only pinned staging (0 upload, 1 download); nullptr on failure   // one grow-only block for the pair-HMM batch call; nullptr on failure
+// pinned host blocks from the first device's pool (pinned_take: nullptr if cudaMallocHost fails; *got = the block's size)
+void *pinned_take(barb200_ctx *ctx, size_t bytes, size_t *got);
+void pinned_give(barb200_ctx *ctx, void *p, size_t bytes);
+// pecan.cu: the context's pair-HMM state (streams, ring scratch, batch group commit), made by barb200_create on the first device
+void **pecan_slot(barb200_ctx *ctx);
+int pecan_create(barb200_ctx *ctx);            // 0 on success; the slot is set either way, so barb200_destroy cleans up
+void pecan_destroy(barb200_ctx *ctx);
 
 }  // namespace barb200
+
+// in a .cu function that returns a BARB200_* code: a failed CUDA call sets the context's message and returns BARB200_ECUDA
+#define CUDA_TRY(ctx, call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { \
+    set_error(ctx, std::string(#call) + ": " + cudaGetErrorString(_e)); return BARB200_ECUDA; } } while (0)

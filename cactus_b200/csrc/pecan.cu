@@ -7,11 +7,13 @@
 // diagonal has <= 96 cells run in 32-thread blocks (24 per SM), all others in 128-thread blocks (6 per SM) whose diagonal
 // ring keeps 320 positions in shared memory and spills the flanks of wider diagonals to an HBM/L2 overflow block (a per-job
 // shift centres the band on the shared part, pecan_cta.cuh). The two launches run concurrently on their own streams.
-// Each resident block owns a slot in HBM for the forward MATCH ring, the ring of complete forward cells and the overflow.
-// Candidate pairs (x, y, log posterior) are appended by the kernel, put into the reference's order of emission on the host,
-// compacted on the device, copied back once and finished on the host with libm's exp (the same function the reference
-// calls), threshold and floor. There is no CPU fallback: the DP only exists as the CUDA kernel below.
+// Each resident block owns a slot of the context's ring scratch in HBM (PecanContext: rings, streams, one run at a time) for
+// the forward MATCH ring, the ring of complete forward cells and the overflow. Candidate pairs (x, y, log posterior) are
+// appended by the kernel, put into the reference's order of emission on the host, compacted on the device, copied back once
+// and finished on the host with libm's exp (the same function the reference calls), threshold and floor. No CPU fallback:
+// the DP only exists as the CUDA kernel below.
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
 #include <omp.h>
 #include <stdio.h>
@@ -93,19 +95,75 @@ extern "C" __global__ void pecan_compact_kernel(const Job *jobs, const int *out_
 }  // namespace pecan
 }  // namespace barb200
 
-#define CUDA_TRY(ctx, call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { \
-    set_error(ctx, std::string(#call) + ": " + cudaGetErrorString(_e)); return BARB200_ECUDA; } } while (0)
+// Block-shape classes by the widest diagonal (file header), chosen by a sweep of alternatives on the benchmark workload. Shared
+// memory per block = 8 * (58 + 11 * rws) bytes: 8.9 KB for the narrow shape, 28.6 KB for the general one; 80 registers.
+struct Class { int max_w, threads, ctas_per_sm, rws; };
+static const Class kClass[] = {{96, 32, 24, 96}, {INT_MAX, 128, 6, 320}};
+static const int kNumClasses = 2;
+
+// The pair-HMM state of a context (pecan_create). `mu` is held by every use of the device below -- a stage's upload, run and
+// collect, and a batch chunk from create to collect -- so one run at a time owns the streams, the events and the ring scratch.
+struct PecanContext {
+    GroupCommit<PecanRequest> group;             // concurrent barb200_pecan_aligned_pairs_batch callers share device batches
+    std::mutex mu;
+    double *scratch = nullptr; size_t scratch_bytes = 0;   // grow-only rings (tens of GB: cudaMalloc of that size costs ~0.2 s)
+    cudaStream_t stream = nullptr, cls[kNumClasses] = {};
+    cudaEvent_t done[kNumClasses] = {}, ev0 = nullptr, ev1 = nullptr;
+};
+static PecanContext &pecan_of(barb200_ctx *ctx) { return *(PecanContext *)*pecan_slot(ctx); }
+
+namespace barb200 {
+int pecan_create(barb200_ctx *ctx) {
+    PecanContext *pc = new PecanContext();
+    *pecan_slot(ctx) = pc;
+    cudaFuncSetAttribute(pecan_posterior_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(pecan_posterior_kernel_r64, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    // wider classes hold longer jobs: they are launched first and at higher priority so that they are resident from the start
+    int prio_lo = 0, prio_hi = 0;
+    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+    bool ok = cudaStreamCreateWithFlags(&pc->stream, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaEventCreate(&pc->ev0) == cudaSuccess && cudaEventCreate(&pc->ev1) == cudaSuccess;
+    for (int c = 0; c < kNumClasses && ok; ++c)
+        ok = cudaStreamCreateWithPriority(&pc->cls[c], cudaStreamNonBlocking, kClass[c].threads <= 32 ? prio_lo : prio_hi) == cudaSuccess &&
+             cudaEventCreateWithFlags(&pc->done[c], cudaEventDisableTiming) == cudaSuccess;
+    return ok ? 0 : -1;
+}
+
+void pecan_destroy(barb200_ctx *ctx) {
+    PecanContext *pc = (PecanContext *)*pecan_slot(ctx);
+    if (!pc) return;
+    if (pc->scratch) cudaFree(pc->scratch);
+    for (int c = 0; c < kNumClasses; ++c) { if (pc->cls[c]) cudaStreamDestroy(pc->cls[c]); if (pc->done[c]) cudaEventDestroy(pc->done[c]); }
+    if (pc->ev0) cudaEventDestroy(pc->ev0);
+    if (pc->ev1) cudaEventDestroy(pc->ev1);
+    if (pc->stream) cudaStreamDestroy(pc->stream);
+    delete pc;
+}
+}  // namespace barb200
+
+// a host staging buffer from the device's pinned pool, so that the copy runs at link speed; pageable memory if the pool cannot grow
+struct Staging {
+    barb200_ctx *ctx; void *pin = nullptr; size_t got = 0; std::vector<uint8_t> own;
+    explicit Staging(barb200_ctx *c) : ctx(c) {}
+    ~Staging() { release(); }
+    Staging(const Staging &) = delete; Staging &operator=(const Staging &) = delete;
+    void *take(size_t bytes) {
+        pin = pinned_take(ctx, bytes, &got);
+        if (pin) return pin;
+        own.resize(bytes);
+        return own.data();
+    }
+    void release() { pinned_give(ctx, pin, got); pin = nullptr; std::vector<uint8_t>().swap(own); }
+};
 
 struct PecanGroup {              // one launch: a class of jobs with one block shape
     std::vector<int> jobs;       // largest first
-    int threads = 32;            // block size
-    int per_sm = 1;              // blocks per SM the shape is sized for
+    int cls = 0;                 // index into kClass
     int ctas = 0;                // resident blocks = slots
     int RW = 32, RWs = 32;       // ring width (the modulus) and its shared-memory part
     unsigned capM = 1024, capF = 1024;   // ring doubles (powers of two)
     size_t slot_doubles = 0, smem_bytes = 0, scratch_off = 0;
     int order_off = 0;           // into d_order
-    cudaStream_t stream = nullptr; cudaEvent_t done = nullptr;
 };
 
 struct barb200_pecan_stage {
@@ -114,20 +172,18 @@ struct barb200_pecan_stage {
     Params devP;
     int64_t n_pairs = 0;
     bool full_cap = false;                       // retry stage: room for every cell
-    bool shared_scratch = false;                 // batch call: rings live in the context's grow-only scratch
     std::vector<SubJob> subs;                    // in pair order
     std::vector<int64_t> pair_first;             // subs of pair i: [pair_first[i], pair_first[i+1])
     std::vector<Job> jobs;
-    std::vector<uint8_t> h_sym;                  // packed symbols 0..4 (kept for re-runs of overflowed jobs)
     std::vector<PecanGroup> groups;
-    int64_t cells = 0, launches = 0, out_total = 0;
-    // device
+    int64_t cells = 0, launches = 0;
+    size_t scratch_bytes = 0;                    // the rings a run takes from the context's scratch
+    // device; a retry stage reads its parent's d_sym, d_meta and d_consts
     uint8_t *d_sym = nullptr; DiagMeta *d_meta = nullptr; int *d_order = nullptr, *d_out_n = nullptr;
-    Job *d_jobs = nullptr; Pair *d_out = nullptr; unsigned *d_counter = nullptr; double *d_consts = nullptr, *d_scratch = nullptr;
-    cudaStream_t stream = nullptr; cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    Job *d_jobs = nullptr; Pair *d_out = nullptr; unsigned *d_counter = nullptr; double *d_consts = nullptr;
     bool ran = false;
     struct Block { void *p; size_t bytes; };
-    std::vector<Block> blocks;                   // device arrays from the context's block cache
+    std::vector<Block> blocks;                   // the stage's own device arrays, from the context's block cache
 };
 
 extern "C" void barb200_pecan_params_default(barb200_pecan_params *p) {
@@ -146,11 +202,6 @@ extern "C" void barb200_pecan_stage_destroy(barb200_pecan_stage *st) {
     if (!st) return;
     cudaSetDevice(ctx_device(st->ctx));
     for (auto &b : st->blocks) device_free(st->ctx, b.p, b.bytes);
-    if (st->d_scratch && !st->shared_scratch) cudaFree(st->d_scratch);
-    for (PecanGroup &g : st->groups) { if (g.stream) cudaStreamDestroy(g.stream); if (g.done) cudaEventDestroy(g.done); }
-    if (st->ev0) cudaEventDestroy(st->ev0);
-    if (st->ev1) cudaEventDestroy(st->ev1);
-    if (st->stream) cudaStreamDestroy(st->stream);
     delete st;
 }
 
@@ -164,11 +215,13 @@ static int plan_params(barb200_ctx *ctx, const barb200_pecan_params *p, PlanPara
     return BARB200_OK;
 }
 
-// build the device side of a stage from st->subs (already split, not yet planned unless bandL is filled)
-// symbols come either from the caller's strings (sx, sy) or, for a retry stage, from the parent stage's packed copy
-static int stage_build(barb200_pecan_stage *st, const char *const *sx, const char *const *sy,
-                       const barb200_pecan_stage *parent, const std::vector<int64_t> *parent_idx) {
+// Build the device side of a stage from st->subs (already split, not yet planned unless bandL is filled). A fresh stage packs
+// the caller's strings (sx, sy) and the band tables straight into one staging block and uploads them. A retry stage re-runs
+// jobs of `parent` with room for every cell: its jobs are copies of the parent's and still index the parent's symbols and band
+// tables on the device, so it uploads only its job table and launch order.
+static int stage_build(barb200_pecan_stage *st, const char *const *sx, const char *const *sy, const barb200_pecan_stage *parent) {
     barb200_ctx *ctx = st->ctx;
+    PecanContext &pc = pecan_of(ctx);
     const int64_t ns = (int64_t)st->subs.size();
     std::string err;
     const int nthr = host_threads(ctx);
@@ -188,69 +241,28 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
     for (int64_t i = 0; i < ns; ++i) {
         SubJob &s = st->subs[i];
         Job &J = st->jobs[i];
-        J.sx_off = sym_off; sym_off += s.lx; J.sy_off = sym_off; sym_off += s.ly;
-        J.band_off = band_off; band_off += (int64_t)s.lx + s.ly + 2;
-        J.lx = s.lx; J.ly = s.ly; J.ragged = s.ragged;
+        if (!parent) { J.sx_off = sym_off; J.sy_off = sym_off + s.lx; J.band_off = band_off; J.lx = s.lx; J.ly = s.ly; J.ragged = s.ragged; }
+        sym_off += (int64_t)s.lx + s.ly; band_off += (int64_t)s.lx + s.ly + 2;
         const int64_t cap = st->full_cap ? s.cells : std::min<int64_t>(s.cells, (int64_t)s.lx + s.ly + 64);
         s.out_cap = (int)cap; J.out_cap = (int)cap; J.out_off = out_off; out_off += cap;
         cells += s.cells;
     }
-    st->cells = cells; st->out_total = out_off;
-    // pack
-    std::vector<uint8_t> &sym = st->h_sym;
-    sym.assign((size_t)std::max<int64_t>(sym_off, 1), 4);
-    std::vector<DiagMeta> meta_own;
-    DiagMeta *meta = nullptr;
-    const size_t meta_n = (size_t)band_off + 1;
-    if (st->shared_scratch) meta = (DiagMeta *)pecan_pinned(ctx, 0, meta_n * sizeof(DiagMeta));     // pinned: the upload runs at link speed
-    if (!meta) { meta_own.resize(meta_n); meta = meta_own.data(); }
-#pragma omp parallel for schedule(dynamic, 16) num_threads(nthr)
-    for (int64_t i = 0; i < ns; ++i) {
-        const SubJob &s = st->subs[i];
-        const Job &J = st->jobs[i];
-        if (parent) {
-            const Job &PJ = parent->jobs[(*parent_idx)[i]];
-            if (s.lx) memcpy(&sym[J.sx_off], &parent->h_sym[PJ.sx_off], s.lx);
-            if (s.ly) memcpy(&sym[J.sy_off], &parent->h_sym[PJ.sy_off], s.ly);
-        } else {
-            const char *px = sx[s.pair] + s.x1, *py = sy[s.pair] + s.y1;
-            for (int k = 0; k < s.lx; ++k) sym[J.sx_off + k] = (uint8_t)sym_of(px[k]);
-            for (int k = 0; k < s.ly; ++k) sym[J.sy_off + k] = (uint8_t)sym_of(py[k]);
-        }
-        const int D = s.lx + s.ly;
-        for (int d = 0; d <= D + 1; ++d) meta[J.band_off + d] = DiagMeta{d <= D ? s.bandL[d] : 0, s.coff[d], s.foff[d], 0};
-    }
-    // classes by the widest diagonal (see the file header); each class is one launch on its own stream
+    st->cells = cells;
+    // classes by the widest diagonal (kClass)
     cudaSetDevice(ctx_device(ctx));
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(ctx, cudaMemGetInfo(&free_b, &total_b));
     const size_t fixed = (size_t)sym_off + (size_t)band_off * 16 + (size_t)ns * (sizeof(Job) + 8) + (size_t)out_off * sizeof(Pair) * 2 + (64 << 20);
     if ((double)fixed > ctx_mem_fraction(ctx) * (double)free_b) { set_error(ctx, "pecan stage does not fit in device memory; submit fewer pairs per call"); return BARB200_ENOMEM; }
     size_t budget = (size_t)(ctx_mem_fraction(ctx) * (double)free_b) - fixed;
-    // shared memory per block = 8 * (58 + 11 * RWs) bytes: 8.9 KB for the narrow shape, 28.6 KB for the general one; 80 registers.
-    // Shapes chosen by a sweep on the benchmark workload (scripts/pecan_sweep.sh sets BARB200_PECAN_CLASSES to compare others).
-    struct Class { int max_w, threads, ctas_per_sm, rws; };
-    std::vector<Class> kClass = {{96, 32, 24, 96}, {0x7fffffff, 128, 6, 320}};
-    if (const char *e = getenv("BARB200_PECAN_CLASSES")) {         // tuning aid: "max_w:threads:blocks_per_sm:shared_ring,..." (last max_w is ignored)
-        kClass.clear();
-        for (const char *q = e; *q;) {
-            int a = 0, b = 0, c = 0, r = 0, n = 0;
-            if (sscanf(q, "%d:%d:%d:%d%n", &a, &b, &c, &r, &n) != 4 || a <= 0 || b < 32 || b > 256 || b % 32 || c <= 0 || r < 32 || 8 * (58 + 11 * (size_t)r) > 200 * 1024) {
-                set_error(ctx, "bad BARB200_PECAN_CLASSES"); return BARB200_EINVAL; }
-            kClass.push_back(Class{a, b, c, r});
-            q += n; if (*q == ',') ++q;
-        }
-        if (kClass.empty()) { set_error(ctx, "bad BARB200_PECAN_CLASSES"); return BARB200_EINVAL; }
-        kClass.back().max_w = 0x7fffffff;
-    }
     st->groups.clear();
-    for (int c = 0; c < (int)kClass.size(); ++c) {
+    for (int c = 0; c < kNumClasses; ++c) {
         PecanGroup g;
         for (int64_t i = 0; i < ns; ++i) if (st->subs[i].max_w <= kClass[c].max_w && (c == 0 || st->subs[i].max_w > kClass[c - 1].max_w)) g.jobs.push_back((int)i);
         if (g.jobs.empty()) continue;
         int64_t spanM = 1, spanF = 1; int rw = 1;
         for (int j : g.jobs) { spanM = std::max(spanM, st->subs[j].span_cells); spanF = std::max(spanF, st->subs[j].span_full_cells); rw = std::max(rw, st->subs[j].max_w); }
-        g.threads = kClass[c].threads; g.per_sm = kClass[c].ctas_per_sm;
+        g.cls = c;
         g.RWs = kClass[c].rws; g.RW = std::max(g.RWs, rw);
         for (int j : g.jobs) st->jobs[j].ring_shift = st->subs[j].ring_center - g.RWs / 2;
         g.capM = pow2ceil((uint64_t)spanM); g.capF = pow2ceil((uint64_t)5 * (uint64_t)spanF);
@@ -276,45 +288,51 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
         g.scratch_off = scratch_doubles; scratch_doubles += g.slot_doubles * (size_t)g.ctas;
         g.order_off = order_off;
         for (int j : g.jobs) order[order_off++] = j;
-        // wider classes hold longer jobs: they are launched first and at higher priority so that they are resident from the start
-        int prio_lo = 0, prio_hi = 0;
-        cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-        CUDA_TRY(ctx, cudaStreamCreateWithPriority(&g.stream, cudaStreamNonBlocking, g.threads <= 32 ? prio_lo : prio_hi));
-        CUDA_TRY(ctx, cudaEventCreateWithFlags(&g.done, cudaEventDisableTiming));
     }
-    const size_t scratch_bytes = scratch_doubles * 8;
+    st->scratch_bytes = std::max<size_t>(scratch_doubles * 8, 8);
     if (getenv("BARB200_DEBUG"))
         for (const PecanGroup &g : st->groups)
             fprintf(stderr, "[barb200] pecan class: %zu jobs, %d threads x %d blocks, ring %d of which %d shared, FM ring %u, FF ring %u doubles, smem %zu B\n",
-                    g.jobs.size(), g.threads, g.ctas, g.RW, g.RWs, g.capM, g.capF, g.smem_bytes);
+                    g.jobs.size(), kClass[g.cls].threads, g.ctas, g.RW, g.RWs, g.capM, g.capF, g.smem_bytes);
     // device arrays
-    Consts C; fill_constants(C);
     auto dev_alloc = [&](void **p, size_t bytes) -> bool {
         if (device_alloc(ctx, p, bytes) != 0) return false;
         st->blocks.push_back(barb200_pecan_stage::Block{*p, bytes});
         return true;
     };
-    const size_t ns1 = (size_t)std::max<int64_t>(ns, 1);
-    if (!dev_alloc((void **)&st->d_sym, sym.size()) || !dev_alloc((void **)&st->d_meta, meta_n * sizeof(DiagMeta)) ||
+    const size_t ns1 = (size_t)std::max<int64_t>(ns, 1), meta_bytes = ((size_t)band_off + 1) * sizeof(DiagMeta);
+    if (parent) { st->d_sym = parent->d_sym; st->d_meta = parent->d_meta; st->d_consts = parent->d_consts; }
+    if ((!parent && (!dev_alloc((void **)&st->d_meta, meta_bytes + (size_t)std::max<int64_t>(sym_off, 1)) || !dev_alloc((void **)&st->d_consts, sizeof(Consts)))) ||
         !dev_alloc((void **)&st->d_order, order.size() * sizeof(int)) || !dev_alloc((void **)&st->d_out_n, ns1 * sizeof(int)) ||
         !dev_alloc((void **)&st->d_jobs, ns1 * sizeof(Job)) || !dev_alloc((void **)&st->d_out, (size_t)std::max<int64_t>(out_off, 1) * sizeof(Pair)) ||
-        !dev_alloc((void **)&st->d_counter, sizeof(unsigned) * (st->groups.size() + 1)) || !dev_alloc((void **)&st->d_consts, sizeof(Consts))) {
+        !dev_alloc((void **)&st->d_counter, sizeof(unsigned) * (st->groups.size() + 1))) {
         set_error(ctx, "device allocation failed (pecan stage)"); return BARB200_ENOMEM;
     }
-    if (st->shared_scratch) {
-        st->d_scratch = (double *)pecan_scratch(ctx, std::max<size_t>(scratch_bytes, 8));
-        if (!st->d_scratch) { set_error(ctx, "device allocation failed (pecan rings)"); return BARB200_ENOMEM; }
-    } else {
-        CUDA_TRY(ctx, cudaMalloc((void **)&st->d_scratch, std::max<size_t>(scratch_bytes, 8)));
+    if (!parent) st->d_sym = (uint8_t *)st->d_meta + meta_bytes;
+    Staging up(ctx);
+    Consts C; fill_constants(C);
+    DiagMeta *meta = nullptr;                    // band tables, then symbols 0..4: the layout of d_meta / d_sym
+    if (!parent) {
+        meta = (DiagMeta *)up.take(meta_bytes + (size_t)sym_off);
+        uint8_t *const sym = (uint8_t *)meta + meta_bytes;
+#pragma omp parallel for schedule(dynamic, 16) num_threads(nthr)
+        for (int64_t i = 0; i < ns; ++i) {
+            const SubJob &s = st->subs[i];
+            const Job &J = st->jobs[i];
+            const char *px = sx[s.pair] + s.x1, *py = sy[s.pair] + s.y1;
+            for (int k = 0; k < s.lx; ++k) sym[J.sx_off + k] = (uint8_t)sym_of(px[k]);
+            for (int k = 0; k < s.ly; ++k) sym[J.sy_off + k] = (uint8_t)sym_of(py[k]);
+            const int D = s.lx + s.ly;
+            for (int d = 0; d <= D + 1; ++d) meta[J.band_off + d] = DiagMeta{d <= D ? s.bandL[d] : 0, s.coff[d], s.foff[d], 0};
+        }
     }
-    CUDA_TRY(ctx, cudaStreamCreateWithFlags(&st->stream, cudaStreamNonBlocking));
-    CUDA_TRY(ctx, cudaEventCreate(&st->ev0)); CUDA_TRY(ctx, cudaEventCreate(&st->ev1));
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->d_sym, sym.data(), sym.size(), cudaMemcpyHostToDevice, st->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->d_meta, meta, meta_n * sizeof(DiagMeta), cudaMemcpyHostToDevice, st->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->d_order, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice, st->stream));
-    if (ns) CUDA_TRY(ctx, cudaMemcpyAsync(st->d_jobs, st->jobs.data(), (size_t)ns * sizeof(Job), cudaMemcpyHostToDevice, st->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(st->d_consts, &C, sizeof(C), cudaMemcpyHostToDevice, st->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(st->d_order, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice, pc.stream));
+    if (ns) CUDA_TRY(ctx, cudaMemcpyAsync(st->d_jobs, st->jobs.data(), (size_t)ns * sizeof(Job), cudaMemcpyHostToDevice, pc.stream));
+    if (!parent) {     // last and in one copy: no copy from the staging block is in flight when an earlier one fails
+        CUDA_TRY(ctx, cudaMemcpyAsync(st->d_consts, &C, sizeof(C), cudaMemcpyHostToDevice, pc.stream));
+        CUDA_TRY(ctx, cudaMemcpyAsync(st->d_meta, meta, meta_bytes + (size_t)sym_off, cudaMemcpyHostToDevice, pc.stream));
+    }
+    CUDA_TRY(ctx, cudaStreamSynchronize(pc.stream));
     st->devP.log_thr_lo = st->P.threshold > 0 ? log(st->P.threshold) - 1e-9 : -INFINITY;
     st->devP.min_diags = (int)st->P.min_diags; st->devP.tb_diags = (int)st->P.tb_diags; st->devP.expansion = (int)st->P.expansion;
     return BARB200_OK;
@@ -323,13 +341,13 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
 static int stage_create_impl(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                              const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                              const int64_t *const *anchors, const int64_t *n_anchor,
-                             const uint8_t *ragged_left, const uint8_t *ragged_right, bool shared_scratch, barb200_pecan_stage **out) {
+                             const uint8_t *ragged_left, const uint8_t *ragged_right, barb200_pecan_stage **out) {
     if (!ctx || !out || n_pairs < 0 || (n_pairs > 0 && (!sx || !sy || !lx || !ly))) { if (ctx) set_error(ctx, "bad argument"); return BARB200_EINVAL; }
     PlanParams P;
     int rc = plan_params(ctx, p, P);
     if (rc) return rc;
     barb200_pecan_stage *st = new barb200_pecan_stage();
-    st->ctx = ctx; st->P = P; st->n_pairs = n_pairs; st->shared_scratch = shared_scratch;
+    st->ctx = ctx; st->P = P; st->n_pairs = n_pairs;
     st->pair_first.assign(n_pairs + 1, 0);
     for (int64_t i = 0; i < n_pairs; ++i) {
         const int64_t na = n_anchor ? n_anchor[i] : 0;
@@ -341,7 +359,7 @@ static int stage_create_impl(barb200_ctx *ctx, const barb200_pecan_params *p, in
         split_pair(P, i, lx[i], ly[i], a, na, ragged_left && ragged_left[i], ragged_right && ragged_right[i], st->subs);
     }
     st->pair_first[n_pairs] = (int64_t)st->subs.size();
-    rc = stage_build(st, sx, sy, nullptr, nullptr);
+    rc = stage_build(st, sx, sy, nullptr);
     if (rc) { barb200_pecan_stage_destroy(st); return rc; }
     *out = st;
     return BARB200_OK;
@@ -352,45 +370,53 @@ extern "C" int barb200_pecan_stage_create(barb200_ctx *ctx, const barb200_pecan_
                                           const int64_t *const *anchors, const int64_t *n_anchor,
                                           const uint8_t *ragged_left, const uint8_t *ragged_right, barb200_pecan_stage **out) {
     if (!ctx) return BARB200_EINVAL;
-    std::lock_guard<std::mutex> lk(device_mutex(ctx));
-    return stage_create_impl(ctx, p, n_pairs, sx, lx, sy, ly, anchors, n_anchor, ragged_left, ragged_right, false, out);
+    std::lock_guard<std::mutex> lk(pecan_of(ctx).mu);
+    return stage_create_impl(ctx, p, n_pairs, sx, lx, sy, ly, anchors, n_anchor, ragged_left, ragged_right, out);
 }
 
 static int stage_run_locked(barb200_pecan_stage *st, float *kernel_ms) {
     barb200_ctx *ctx = st->ctx;
+    PecanContext &pc = pecan_of(ctx);
     cudaSetDevice(ctx_device(ctx));
-    // per device, and cheap: set on every run (a process may hold contexts on several GPUs)
-    cudaFuncSetAttribute(pecan_posterior_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(pecan_posterior_kernel_r64, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    CUDA_TRY(ctx, cudaMemsetAsync(st->d_counter, 0, sizeof(unsigned) * (st->groups.size() + 1), st->stream));
-    CUDA_TRY(ctx, cudaEventRecord(st->ev0, st->stream));
+    if (pc.scratch_bytes < st->scratch_bytes) {      // grow the context's rings
+        cudaFree(pc.scratch);
+        pc.scratch_bytes = 0;
+        if (cudaMalloc((void **)&pc.scratch, st->scratch_bytes) != cudaSuccess) {
+            cudaGetLastError(); pc.scratch = nullptr;
+            set_error(ctx, "device allocation failed (pecan rings)"); return BARB200_ENOMEM;
+        }
+        pc.scratch_bytes = st->scratch_bytes;
+    }
+    CUDA_TRY(ctx, cudaMemsetAsync(st->d_counter, 0, sizeof(unsigned) * (st->groups.size() + 1), pc.stream));
+    CUDA_TRY(ctx, cudaEventRecord(pc.ev0, pc.stream));
     st->launches = 0;
-    for (size_t gq = st->groups.size(); gq-- > 0;) {          // widest class first
-        const size_t gi = gq;
+    for (size_t gi = st->groups.size(); gi-- > 0;) {          // widest class first
         const PecanGroup &g = st->groups[gi];
+        const Class &K = kClass[g.cls];
+        cudaStream_t cs = pc.cls[g.cls];
         KernelArgs A;
         A.jobs = st->d_jobs; A.order = st->d_order + g.order_off; A.n_jobs = (int)g.jobs.size();
         A.sym = st->d_sym; A.meta = st->d_meta; A.out = st->d_out; A.out_n = st->d_out_n;
-        A.counter = st->d_counter + gi; A.consts = st->d_consts; A.scratch = st->d_scratch + g.scratch_off; A.slot_doubles = g.slot_doubles;
+        A.counter = st->d_counter + gi; A.consts = st->d_consts; A.scratch = pc.scratch + g.scratch_off; A.slot_doubles = g.slot_doubles;
         A.maskM = g.capM - 1; A.maskF = g.capF - 1; A.RW = g.RW; A.RWs = g.RWs; A.P = st->devP;
-        CUDA_TRY(ctx, cudaStreamWaitEvent(g.stream, st->ev0, 0));
-        if (g.threads * g.per_sm > 768) pecan_posterior_kernel_r64<<<g.ctas, g.threads, g.smem_bytes, g.stream>>>(A);
-        else pecan_posterior_kernel<<<g.ctas, g.threads, g.smem_bytes, g.stream>>>(A);
+        CUDA_TRY(ctx, cudaStreamWaitEvent(cs, pc.ev0, 0));
+        if (K.threads * K.ctas_per_sm > 768) pecan_posterior_kernel_r64<<<g.ctas, K.threads, g.smem_bytes, cs>>>(A);
+        else pecan_posterior_kernel<<<g.ctas, K.threads, g.smem_bytes, cs>>>(A);
         CUDA_TRY(ctx, cudaGetLastError());
-        CUDA_TRY(ctx, cudaEventRecord(g.done, g.stream));
-        CUDA_TRY(ctx, cudaStreamWaitEvent(st->stream, g.done, 0));
+        CUDA_TRY(ctx, cudaEventRecord(pc.done[g.cls], cs));
+        CUDA_TRY(ctx, cudaStreamWaitEvent(pc.stream, pc.done[g.cls], 0));
         ++st->launches;
     }
-    CUDA_TRY(ctx, cudaEventRecord(st->ev1, st->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(st->stream));
-    if (kernel_ms) CUDA_TRY(ctx, cudaEventElapsedTime(kernel_ms, st->ev0, st->ev1));
+    CUDA_TRY(ctx, cudaEventRecord(pc.ev1, pc.stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(pc.stream));
+    if (kernel_ms) CUDA_TRY(ctx, cudaEventElapsedTime(kernel_ms, pc.ev0, pc.ev1));
     st->ran = true;
     return BARB200_OK;
 }
 
 extern "C" int barb200_pecan_stage_run(barb200_pecan_stage *st, float *kernel_ms) {
     if (!st) return BARB200_EINVAL;
-    std::lock_guard<std::mutex> lk(device_mutex(st->ctx));
+    std::lock_guard<std::mutex> lk(pecan_of(st->ctx).mu);
     return stage_run_locked(st, kernel_ms);
 }
 
@@ -414,21 +440,21 @@ static int stage_collect(barb200_pecan_stage *st, std::vector<std::vector<Pair>>
         dst_off[i + 1] = dst_off[i] + (over ? 0 : out_n[i]);
     }
     const long long total = dst_off[ns];
-    std::vector<Pair> flat_own;
-    Pair *flat = st->shared_scratch ? (Pair *)pecan_pinned(ctx, 1, sizeof(Pair) * (size_t)std::max<long long>(total, 1)) : nullptr;
-    if (!flat) { flat_own.resize((size_t)std::max<long long>(total, 1)); flat = flat_own.data(); }
+    Staging down(ctx);
+    Pair *const flat = total > 0 ? (Pair *)down.take(sizeof(Pair) * (size_t)total) : nullptr;
     if (total > 0) {
         long long *d_dst_off = nullptr; Pair *d_flat = nullptr;
         if (device_alloc(ctx, (void **)&d_dst_off, sizeof(long long) * (ns + 1)) != 0) { set_error(ctx, "device allocation failed (compact offsets)"); return BARB200_ENOMEM; }
         cudaError_t e = cudaSuccess;
         if (device_alloc(ctx, (void **)&d_flat, sizeof(Pair) * (size_t)total) != 0) {
             device_free(ctx, d_dst_off, sizeof(long long) * (ns + 1)); set_error(ctx, "device allocation failed (compact output)"); return BARB200_ENOMEM; }
-        cudaMemcpyAsync(d_dst_off, dst_off.data(), sizeof(long long) * (ns + 1), cudaMemcpyHostToDevice, st->stream);
+        cudaStream_t s = pecan_of(ctx).stream;
+        cudaMemcpyAsync(d_dst_off, dst_off.data(), sizeof(long long) * (ns + 1), cudaMemcpyHostToDevice, s);
         const int grid = (int)std::min<int64_t>(ns, (int64_t)ctx_sm_count(ctx) * 16);
-        pecan_compact_kernel<<<grid, 128, 0, st->stream>>>(st->d_jobs, st->d_out_n, d_dst_off, st->d_out, d_flat, (int)ns);
+        pecan_compact_kernel<<<grid, 128, 0, s>>>(st->d_jobs, st->d_out_n, d_dst_off, st->d_out, d_flat, (int)ns);
         ++st->launches;
-        cudaMemcpyAsync(flat, d_flat, sizeof(Pair) * (size_t)total, cudaMemcpyDeviceToHost, st->stream);
-        e = cudaStreamSynchronize(st->stream);
+        cudaMemcpyAsync(flat, d_flat, sizeof(Pair) * (size_t)total, cudaMemcpyDeviceToHost, s);
+        e = cudaStreamSynchronize(s);
         device_free(ctx, d_dst_off, sizeof(long long) * (ns + 1)); device_free(ctx, d_flat, sizeof(Pair) * (size_t)total);
         if (e != cudaSuccess) { set_error(ctx, std::string("pecan compaction: ") + cudaGetErrorString(e)); return BARB200_ECUDA; }
     }
@@ -455,12 +481,13 @@ static int stage_collect(barb200_pecan_stage *st, std::vector<std::vector<Pair>>
             v.swap(w);
         }
     }
+    down.release();
     if (!retry.empty()) {
         if (st->full_cap) { set_error(ctx, "pecan: output overflow with full capacity (internal error)"); return BARB200_EJOB; }
         barb200_pecan_stage *rs = new barb200_pecan_stage();
-        rs->ctx = ctx; rs->P = st->P; rs->n_pairs = st->n_pairs; rs->full_cap = true;
-        for (int64_t i : retry) rs->subs.push_back(st->subs[i]);
-        int rc = stage_build(rs, nullptr, nullptr, st, &retry);
+        rs->ctx = ctx; rs->P = st->P; rs->full_cap = true;
+        for (int64_t i : retry) { rs->subs.push_back(st->subs[i]); rs->jobs.push_back(st->jobs[i]); }
+        int rc = stage_build(rs, nullptr, nullptr, st);
         if (rc == BARB200_OK) rc = stage_run_locked(rs, nullptr);
         std::vector<std::vector<Pair>> sub2;
         if (rc == BARB200_OK) rc = stage_collect(rs, sub2);
@@ -516,41 +543,11 @@ extern "C" int barb200_pecan_stage_fetch(barb200_pecan_stage *st, int64_t **trip
     std::vector<std::vector<Pair>> per_sub;
     int rc;
     {
-        std::lock_guard<std::mutex> lk(device_mutex(st->ctx));
+        std::lock_guard<std::mutex> lk(pecan_of(st->ctx).mu);
         rc = stage_collect(st, per_sub);
     }
     if (rc) return rc;
     return finish_pairs(st, per_sub, triples_out, n_out, posteriors_out, cells_out);
-}
-
-namespace barb200 { GroupCommit<PecanRequest> &pecan_group(barb200_ctx *ctx); }   // barb200.cu
-
-static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
-                           const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
-                           const int64_t *const *anchors, const int64_t *n_anchor,
-                           const uint8_t *ragged_left, const uint8_t *ragged_right,
-                           int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out);
-
-// Concurrent callers (one per OpenMP thread of bar(), bar/impl/bar.c:90-94) share device batches: whatever is waiting when the
-// device becomes free runs as ONE batch (group_commit.h, batch_merge.h); a single caller runs its own request unchanged.
-extern "C" int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
-                                                 const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
-                                                 const int64_t *const *anchors, const int64_t *n_anchor,
-                                                 const uint8_t *ragged_left, const uint8_t *ragged_right,
-                                                 int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out) {
-    if (!ctx || !p || !triples_out || !n_out || n_pairs < 0 || (n_pairs > 0 && (!sx || !sy || !lx || !ly))) { if (ctx) set_error(ctx, "bad argument"); return BARB200_EINVAL; }
-    PecanRequest r;
-    r.p = *p; r.n = n_pairs; r.sx = sx; r.lx = lx; r.sy = sy; r.ly = ly; r.anchors = anchors; r.n_anchor = n_anchor;
-    r.ragged_left = ragged_left; r.ragged_right = ragged_right;
-    r.triples_out = triples_out; r.n_out = n_out; r.posteriors_out = posteriors_out; r.cells_out = cells_out;
-    pecan_group(ctx).submit(&r, pecan_can_merge, [ctx](std::vector<PecanRequest *> &batch) {
-        run_pecan_group(batch, [ctx](const barb200_pecan_params *pp, int64_t n, const char *const *a, const int64_t *la, const char *const *b, const int64_t *lb,
-                                     const int64_t *const *an, const int64_t *na, const uint8_t *rl, const uint8_t *rr, int64_t **trip, int64_t *no,
-                                     double **post, int64_t *cells) {
-            return pecan_batch_now(ctx, pp, n, a, la, b, lb, an, na, rl, rr, trip, no, post, cells);
-        });
-    });
-    return r.rc;
 }
 
 static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
@@ -567,10 +564,10 @@ static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int6
         while (i1 < n_pairs && (i1 == i0 || rec + lx[i1] + ly[i1] + 64 <= kChunkRecords)) { rec += lx[i1] + ly[i1] + 64; ++i1; }
         barb200_pecan_stage *st = nullptr;
         const double t0 = omp_get_wtime();
-        std::unique_lock<std::mutex> lk(device_mutex(ctx));      // the chunk owns the context's ring scratch from create to collect
+        std::unique_lock<std::mutex> lk(pecan_of(ctx).mu);      // held from create to collect, like a stage's three calls
         int rc = stage_create_impl(ctx, p, i1 - i0, sx + i0, lx + i0, sy + i0, ly + i0, anchors ? anchors + i0 : nullptr,
                                    n_anchor ? n_anchor + i0 : nullptr, ragged_left ? ragged_left + i0 : nullptr,
-                                   ragged_right ? ragged_right + i0 : nullptr, true, &st);
+                                   ragged_right ? ragged_right + i0 : nullptr, &st);
         const double t1 = omp_get_wtime();
         if (rc == BARB200_OK) rc = stage_run_locked(st, nullptr);
         const double t2 = omp_get_wtime();
@@ -588,6 +585,28 @@ static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int6
         i0 = i1;
     }
     return BARB200_OK;
+}
+
+// Concurrent callers (one per OpenMP thread of bar(), bar/impl/bar.c:90-94) share device batches: whatever is waiting when the
+// device becomes free runs as ONE batch (group_commit.h, batch_merge.h); a single caller runs its own request unchanged.
+extern "C" int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
+                                                 const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
+                                                 const int64_t *const *anchors, const int64_t *n_anchor,
+                                                 const uint8_t *ragged_left, const uint8_t *ragged_right,
+                                                 int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out) {
+    if (!ctx || !p || !triples_out || !n_out || n_pairs < 0 || (n_pairs > 0 && (!sx || !sy || !lx || !ly))) { if (ctx) set_error(ctx, "bad argument"); return BARB200_EINVAL; }
+    PecanRequest r;
+    r.p = *p; r.n = n_pairs; r.sx = sx; r.lx = lx; r.sy = sy; r.ly = ly; r.anchors = anchors; r.n_anchor = n_anchor;
+    r.ragged_left = ragged_left; r.ragged_right = ragged_right;
+    r.triples_out = triples_out; r.n_out = n_out; r.posteriors_out = posteriors_out; r.cells_out = cells_out;
+    pecan_of(ctx).group.submit(&r, pecan_can_merge, [ctx](std::vector<PecanRequest *> &batch) {
+        run_pecan_group(batch, [ctx](const barb200_pecan_params *pp, int64_t n, const char *const *a, const int64_t *la, const char *const *b, const int64_t *lb,
+                                     const int64_t *const *an, const int64_t *na, const uint8_t *rl, const uint8_t *rr, int64_t **trip, int64_t *no,
+                                     double **post, int64_t *cells) {
+            return pecan_batch_now(ctx, pp, n, a, la, b, lb, an, na, rl, rr, trip, no, post, cells);
+        });
+    });
+    return r.rc;
 }
 
 extern "C" int barb200_pecan_band(int64_t lx, int64_t ly, const int64_t *anchors, int64_t n_anchor, int64_t expansion, int64_t *xmy_l, int64_t *xmy_r) {
