@@ -42,10 +42,11 @@ extern "C" __global__ void poa_msa_kernel_t1024(const BatchArgs A);
 }
 typedef void (*poa_kernel_fn)(const barb200::BatchArgs);
 // CTA-size classes: a CTA of T threads sweeps rows of up to 16*T columns (query length + 1)
-// scratch = dynamic shared memory per CTA for the topological sort, sized so that the class's CTAs per SM still fit
+// scratch = dynamic shared memory per CTA (poa_kernel.cuh: poa_scratch_bytes)
 static const struct { int T; poa_kernel_fn fn; int scratch; } kKernels[] = {
-    {32, barb200::poa_msa_kernel_t32, 10 * 1024}, {64, barb200::poa_msa_kernel_t64, 24 * 1024}, {128, barb200::poa_msa_kernel_t128, 40 * 1024},
-    {256, barb200::poa_msa_kernel_t256, 96 * 1024}, {640, barb200::poa_msa_kernel_t640, 200 * 1024}, {1024, barb200::poa_msa_kernel_t1024, 200 * 1024}};
+    {32, barb200::poa_msa_kernel_t32, barb200::poa_scratch_bytes(32)}, {64, barb200::poa_msa_kernel_t64, barb200::poa_scratch_bytes(64)},
+    {128, barb200::poa_msa_kernel_t128, barb200::poa_scratch_bytes(128)}, {256, barb200::poa_msa_kernel_t256, barb200::poa_scratch_bytes(256)},
+    {640, barb200::poa_msa_kernel_t640, barb200::poa_scratch_bytes(640)}, {1024, barb200::poa_msa_kernel_t1024, barb200::poa_scratch_bytes(1024)}};
 static const int kNumKernels = 6;
 static const int kMaxDevices = 8;
 using namespace barb200;
@@ -498,6 +499,9 @@ static int plan_stage(barb200_stage *st) {
         Y.slot_bytes = align_up(o, 256);
         B.T = kKernels[B.cls].T; B.dyn_smem = kKernels[B.cls].scratch;
         if (getenv("BARB200_SCRATCH_KB")) B.dyn_smem = (size_t)atoi(getenv("BARB200_SCRATCH_KB")) * 1024;   // tuning aid
+        // never below the sweep's ring, which the kernel uses without a run-time check (the topological sort and the MSA ranking
+        // fit whatever is left, falling back to global memory)
+        B.dyn_smem = std::max(B.dyn_smem, (size_t)poa_ring_bytes(B.T));
         int per_sm = 0;
         CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kKernels[B.cls].fn, B.T, B.dyn_smem));
         if (per_sm < 1) { set_error(ctx, "kernel does not fit on an SM with the requested configuration"); return BARB200_EINVAL; }

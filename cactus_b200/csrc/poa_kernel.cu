@@ -15,8 +15,9 @@
 //     row just computed therefore stay in the owning thread's registers and feed the next row without touching
 //     memory when the predecessor is the previous row (the common case in a near-linear graph); only H[16t-1]
 //     comes from the neighbour thread (warp shuffle; one shared-memory word per warp boundary). Predecessors
-//     further back are read from the planes in global memory (L2), one 16-byte chunk per thread and instruction, a warp's
-//     chunk 512 contiguous bytes;
+//     two rows back (every substitution bubble and deletion makes such rows) are read from a ring of the last two rows in
+//     the CTA's dynamic shared memory, where the class's scratch holds two rows; older ones from the planes in global memory
+//     (L2), one 16-byte chunk per thread and instruction, a warp's chunk 512 contiguous bytes;
 //   * the max-plus recurrence of the two insertion states F1/F2 along the row is turned into a plain prefix
 //     maximum by the substitution A[k] = H'[k] - oe + (k+1)*e  =>  F[j] = max_{k<j} A[k] - j*e: 16 serial cells per
 //     thread, a warp shuffle scan over the 32 thread aggregates, a redux over the warp aggregates staged in
@@ -45,6 +46,7 @@ struct KShared {
     int wF[2][2][32];      // [row parity][plane F1/F2][warp] block scan staging
     int wM[2][4][32];      // [row parity][max, leftmost, rightmost, H of the warp's last column][warp]
     RowRec rec[2];         // [row parity] the sweep's row record, fetched one row ahead
+    RowInfo ring_info[2];  // [row parity] band of the row held in that slot of the shared-memory ring (dp_sweep)
 };
 
 __device__ __forceinline__ int4 ld4cg(const int *p) { return __ldcg(reinterpret_cast<const int4 *>(p)); }
@@ -55,6 +57,24 @@ __device__ __forceinline__ int4 ld4cg(const int *p) { return __ldcg(reinterpret_
 __device__ __forceinline__ void st4(int *p, int a, int b, int c, int d) {
     asm volatile("st.global.v4.s32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+// the same 16-byte chunks in the shared-memory ring of the sweep: one STS.128 / LDS.128 per chunk, a warp's access 512
+// contiguous bytes (conflict-free); tests/test_sweep_ring_sass.py pins them. a: shared-window byte address
+__device__ __forceinline__ void sts4(unsigned a, int x, int y, int z, int w) {
+    asm volatile("st.shared.v4.s32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+__device__ __forceinline__ int4 lds4(unsigned a) {
+    int4 v;
+    asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ int lds1(unsigned a) {
+    int v;
+    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+// the value of v, opaque to the compiler: what is computed from it in the row loop stays there. The 16 per-column gap offsets
+// j*e of each plane, hoisted out of the loop, hold 32 registers across it and are spilled and reloaded in every row
+__device__ __forceinline__ int opaque(int v) { asm volatile("" : "+r"(v)); return v; }
 __device__ __forceinline__ int max3(int a, int b, int c) { return max(max(a, b), c); }
 // 16-byte global -> shared copy that bypasses the registers (completes at cp_async_wait_all)
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
@@ -89,12 +109,28 @@ __device__ __forceinline__ void row_pass1(int (&H)[CPT], int (&E1)[CPT], int (&E
     }
 }
 
+// folds chunk oc of a predecessor row (4 H values, 4 D codes) into my columns' candidates: H[e+1] <- the M input H_pred[e],
+// E1 / E2 <- max with the decoded E values. ROW0: the predecessor may be row 0, whose D holds the E_NEG16 sentinel (every
+// other row's codes lie in [e, oe], poa_types.h: DpState)
+template <bool ROW0>
+__device__ __forceinline__ void pred_chunk(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], int oc, int4 h4, int4 d4, int NEG) {
+    const int h[CHUNK] = {h4.x, h4.y, h4.z, h4.w}, dv[CHUNK] = {d4.x, d4.y, d4.z, d4.w};
+#pragma unroll
+    for (int u = 0; u < CHUNK; ++u) {
+        const int e = oc * CHUNK + u;
+        const int c1 = dv[u] & 0xffff, c2 = (int)((unsigned)dv[u] >> 16);
+        if (e + 1 < CPT) H[e + 1] = max(H[e + 1], h[u]);
+        E1[e] = max(E1[e], ROW0 && c1 == E_NEG16 ? NEG : h[u] - c1); E2[e] = max(E2[e], ROW0 && c2 == E_NEG16 ? NEG : h[u] - c2);
+    }
+}
+
 // MODE 0: all of the warp's active columns are inside the band; 1: some lie left (or left and right) of it -- every value
 // of an outside cell is forced to inf_min; 2: some lie right of it only -- nothing in the band depends on those cells
 // and the traceback never reads the F planes outside the band, so only H / E1 / E2 are forced (they feed later rows).
-template <int MODE>
+// RING_NT: threads per CTA if the row also goes to the shared-memory ring (rs: address of my chunk 0 of the slot), else 0
+template <int MODE, int RING_NT>
 __device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], int P1, int P2, int j0, int beg, int end, int NEG,
-                                          int je1, int je2, int e1, int e2, int o1, int o2, int *tp, int64_t cs, int &tmax) {
+                                          int je1, int je2, int e1, int e2, int o1, int o2, int *tp, int64_t cs, unsigned rs, int &tmax) {
     const int oe1 = o1 + e1, oe2 = o2 + e2;
     // one H chunk and one D chunk per 4 cells (tp: the thread's chunk 0, cs: ints between chunks; poa_types.h: DpState)
 #pragma unroll
@@ -121,6 +157,10 @@ __device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E
         }
         st4(tp + oc * cs, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
         st4(tp + (CPT / CHUNK + oc) * cs, dd[0], dd[1], dd[2], dd[3]);
+        if (RING_NT) {
+            sts4(rs + oc * RING_NT * 16, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
+            sts4(rs + (CPT / CHUNK + oc) * RING_NT * 16, dd[0], dd[1], dd[2], dd[3]);
+        }
     }
 }
 
@@ -140,9 +180,21 @@ __device__ __forceinline__ void row_argmax(const int (&H)[CPT], int v, int j0, i
 // ---------------------------------------------------------------------------------------------------------
 // banded convex-gap DP of query q[1..L] against the sorted graph. All threads of the CTA; L + 1 <= 16 * blockDim.x.
 // Returns the number of banded cells (sum of dp_end-dp_beg+1), or -1 if the planes outgrew the slot.
+//
+// The ring: where the class's dynamic shared memory holds two rows (every class but t1024), each row also goes to slot
+// r & 1 of a ring there, chunk-major like the planes but with a block for every thread of the CTA: chunk c of thread t at
+// int (c * NT + t) * CHUNK of the slot, so a warp's access to a chunk is 512 contiguous bytes. ring_info[r & 1] holds the
+// row's band. A predecessor at r - 2 is read from there instead of from L2. No extra barrier guards the slots: row r reads
+// slot r & 1 (row r - 2) before its first barrier and overwrites it only in its second pass, after that barrier; tid 0 writes
+// ring_info[r & 1] after the second barrier, and row r + 1, which reads the other slot, starts after both. Rows r - 1 and
+// r - 2 wrote their slots before barriers row r has already passed.
 // ---------------------------------------------------------------------------------------------------------
-__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L, uint2 *qsm) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+template <int NT>
+__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L, uint2 *qsm, unsigned ring) {
+    constexpr int RING_NT = poa_ring_bytes(NT) ? NT : 0;                        // a compile-time property of the class
+    constexpr unsigned SLOT = NT * TB * sizeof(int), RCS = NT * 16;              // ring bytes per slot, between chunks
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = NT >> 5;
+    const unsigned my_ring = ring + tid * 16;                                       // my chunk 0 of slot 0
     const PoaParams &P = A.P;
     // slot arrays addressed from the kernel parameters (not through the pointers cached in shared memory), so that the
     // compiler knows they are global memory and emits LDG/STG instead of generic accesses
@@ -158,7 +210,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
     const int w = P.wb + (int)(P.wf * L);                                    // abpoa_align_simd.c:474
     const int pn_shift = reference_lane_count(P, L, node_n) == 16 ? 4 : 3;
     static_assert(CPT == 16, "shifts below assume 16 columns per thread");
-    const int j0 = tid * CPT, je1 = j0 * e1, je2 = j0 * e2;
+    const int j0 = tid * CPT;
 
     // query codes of my 16 columns, 4 bits each (column j scores against q_j = qg[j-1]; column 0 and columns past the
     // query score 0, abpoa_align_simd.c:536)
@@ -203,8 +255,18 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
                 st4(tp + (CPT / CHUNK + oc) * cs, D[oc * CHUNK], D[oc * CHUNK + 1], D[oc * CHUNK + 2], D[oc * CHUNK + 3]);
             }
         }
+        if (RING_NT) {
+#pragma unroll
+            for (int oc = 0; oc < CPT / CHUNK; ++oc) {
+                sts4(my_ring + oc * RCS, H[oc * CHUNK], H[oc * CHUNK + 1], H[oc * CHUNK + 2], H[oc * CHUNK + 3]);
+                sts4(my_ring + (CPT / CHUNK + oc) * RCS, D[oc * CHUNK], D[oc * CHUNK + 1], D[oc * CHUNK + 2], D[oc * CHUNK + 3]);
+            }
+        }
         if (lane == 31) S.wM[0][3][warp] = H[CPT - 1];
-        if (tid == 0) { RowInfo ri; ri.beg = 0; ri.end = prev_end; ri.left = 0; ri.right = 0; info[0] = ri; row_off[0] = 0; }
+        if (tid == 0) {
+            RowInfo ri; ri.beg = 0; ri.end = prev_end; ri.left = 0; ri.right = 0; info[0] = ri; row_off[0] = 0;
+            if (RING_NT) S.ring_info[0] = ri;
+        }
         cur_blk = nTs; cells = prev_end + 1;
         if (tid == 0) { cp_async16(&S.rec[1], rec_tab + (R > 1 ? 1 : 0)); cp_async_wait_all(); }
     }
@@ -228,6 +290,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
                 const int p = k == 0 ? rec.pre0 : pre_row[rec.pre_off + k];
                 int pl, pr, pb;
                 if (p == r - 1) { pl = prev_left; pr = prev_right; pb = prev_beg; has_prev = true; }
+                else if (RING_NT && p == r - 2) { const RowInfo pi = S.ring_info[par]; pl = pi.left; pr = pi.right; pb = pi.beg; }
                 else { const RowInfo pi = info[p]; pl = pi.left; pr = pi.right; pb = pi.beg; }
                 maxL = min(maxL, pl + 1); maxR = max(maxR, pr + 1); min_pre_beg = min(min_pre_beg, pb);
             }
@@ -262,36 +325,44 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
                 for (int e = 0; e < CPT; ++e) { H[e] = NEG; E1[e] = NEG; E2[e] = NEG; }
                 if (has_prev) H[0] = hl;
             }
-            // predecessors further back: from the planes in global memory
+            // predecessors further back: row r - 2 from the ring, older ones from the planes in global memory
 #pragma unroll 1
             for (int k = only_prev ? npre : 0; k < npre; ++k) {
                 const int p = k == 0 ? rec.pre0 : pre_row[rec.pre_off + k];
                 if (p == r - 1) continue;
+                if (RING_NT && p == r - 2) {
+                    const RowInfo pi = S.ring_info[par];
+                    const int pt0 = pi.beg >> 4, pnT = (pi.end >> 4) - pt0 + 1, ptt = tid - pt0;
+                    const unsigned rs = my_ring + par * SLOT;
+                    if (ptt >= 0 && ptt < pnT) {
+                        if (p == 0) {                                             // uniform across the CTA
+#pragma unroll
+                            for (int oc = 0; oc < CPT / CHUNK; ++oc) pred_chunk<true>(H, E1, E2, oc, lds4(rs + oc * RCS), lds4(rs + (CPT / CHUNK + oc) * RCS), NEG);
+                        } else {
+#pragma unroll
+                            for (int oc = 0; oc < CPT / CHUNK; ++oc) pred_chunk<false>(H, E1, E2, oc, lds4(rs + oc * RCS), lds4(rs + (CPT / CHUNK + oc) * RCS), NEG);
+                        }
+                    }
+                    // H[16*tid - 1]: the last H (chunk 3) of the left neighbour's block
+                    if (ptt >= 1 && ptt <= pnT) H[0] = max(H[0], lds1(rs + (CPT / CHUNK - 1) * RCS - 4));
+                    continue;
+                }
                 const RowInfo pi = info[p];
                 const int pt0 = pi.beg >> 4, pnT = (pi.end >> 4) - pt0 + 1, ptt = tid - pt0, pnTs = row_blocks(pi.beg, pi.end);
                 const int *Hp = planes + row_off[p] + chunk_index(pnTs, tid - row_t0(pi.beg), 0);   // my block of row p (if stored)
                 const int64_t pcs = chunk_index(pnTs, 0, 1);
                 if (ptt >= 0 && ptt < pnT) {
 #pragma unroll
-                    for (int oc = 0; oc < CPT / CHUNK; ++oc) {
-                        const int4 h4 = ld4cg(Hp + oc * pcs), d4 = ld4cg(Hp + (CPT / CHUNK + oc) * pcs);
-                        const int h[CHUNK] = {h4.x, h4.y, h4.z, h4.w}, dv[CHUNK] = {d4.x, d4.y, d4.z, d4.w};
-#pragma unroll
-                        for (int u = 0; u < CHUNK; ++u) {
-                            const int e = oc * CHUNK + u;
-                            const int c1 = dv[u] & 0xffff, c2 = (int)((unsigned)dv[u] >> 16);
-                            if (e + 1 < CPT) H[e + 1] = max(H[e + 1], h[u]);
-                            E1[e] = max(E1[e], c1 == E_NEG16 ? NEG : h[u] - c1); E2[e] = max(E2[e], c2 == E_NEG16 ? NEG : h[u] - c2);
-                        }
-                    }
+                    for (int oc = 0; oc < CPT / CHUNK; ++oc) pred_chunk<true>(H, E1, E2, oc, ld4cg(Hp + oc * pcs), ld4cg(Hp + (CPT / CHUNK + oc) * pcs), NEG);
                 }
                 // H[16*tid - 1]: the last H (chunk 3) of the left neighbour's block
                 if (ptt >= 1 && ptt <= pnT) H[0] = max(H[0], __ldcg(Hp - CHUNK + (CPT / CHUNK - 1) * pcs + CHUNK - 1));
             }
             const uint2 q2 = qsm[tid];
             const uint32_t qr[2] = {q2.x, q2.y};
-            if (wmode != 1) row_pass1<false>(H, E1, E2, mrow, qr, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
-            else row_pass1<true>(H, E1, E2, mrow, qr, j0, beg, end, NEG, je1, je2, e1, e2, agg1, agg2);
+            const int pe1 = opaque(e1), pe2 = opaque(e2);
+            if (wmode != 1) row_pass1<false>(H, E1, E2, mrow, qr, j0, beg, end, NEG, j0 * pe1, j0 * pe2, pe1, pe2, agg1, agg2);
+            else row_pass1<true>(H, E1, E2, mrow, qr, j0, beg, end, NEG, j0 * pe1, j0 * pe2, pe1, pe2, agg1, agg2);
         }
         // ---- exclusive prefix maximum over the row: warp shuffle scan + redux over warp aggregates ----
         int inc1 = agg1, inc2 = agg2;
@@ -317,10 +388,12 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         {
             int *tp = planes + (int64_t)cur_blk * TB + chunk_index(nTs, tts, 0);
             const int64_t cs = chunk_index(nTs, 0, 1);
+            const unsigned rs = my_ring + par * SLOT;
             if (active) {
-                if (wmode == 0) row_pass2<0>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
-                else if (wmode == 2) row_pass2<2>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
-                else row_pass2<1>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, e1, e2, P.o1, P.o2, tp, cs, tmax);
+                const int pe1 = opaque(e1), pe2 = opaque(e2), je1 = j0 * pe1, je2 = j0 * pe2;
+                if (wmode == 0) row_pass2<0, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
+                else if (wmode == 2) row_pass2<2, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
+                else row_pass2<1, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
             } else if ((unsigned)tts < (unsigned)nTs) store_pad(tp, cs, NEG);
         }
         // ---- left/right-most argmax of H over the band (simd_abpoa_max_in_row, :1107-1119) ----
@@ -344,7 +417,10 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
             prev_left = __reduce_min_sync(FULL, l); prev_right = __reduce_max_sync(FULL, rr);
         }
         prev_beg = beg; prev_end = end; prev_active = active;
-        if (tid == 0) { RowInfo ri; ri.beg = beg; ri.end = end; ri.left = prev_left; ri.right = prev_right; info[r] = ri; row_off[r] = (int64_t)cur_blk * TB; }
+        if (tid == 0) {
+            RowInfo ri; ri.beg = beg; ri.end = end; ri.left = prev_left; ri.right = prev_right; info[r] = ri; row_off[r] = (int64_t)cur_blk * TB;
+            if (RING_NT) S.ring_info[par] = ri;
+        }
         cur_blk += nTs; cells += end - beg + 1;
     }
     __syncthreads();
@@ -375,7 +451,7 @@ __device__ __forceinline__ void carve(KShared &S, const BatchArgs &A, int slot) 
 
 template <int NT>
 __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
-    extern __shared__ __align__(16) unsigned char dyn_smem[];    // scratch of the topological sort (poa_cta.cuh)
+    extern __shared__ __align__(16) unsigned char dyn_smem[];    // scratch of the topological sort (poa_cta.cuh), the sweep's row ring
     __shared__ KShared S;
     __shared__ uint2 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
     const int tid = threadIdx.x;
@@ -416,7 +492,7 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
                 PHASE_TICK(PH_FUSE);
             } else {
                 long long c = -2;
-                if (L + 1 <= CPT * (int)blockDim.x) c = dp_sweep(S, A, q, L, qsm);
+                if (L + 1 <= CPT * (int)blockDim.x) c = dp_sweep<NT>(S, A, q, L, qsm, (unsigned)__cvta_generic_to_shared(dyn_smem));
                 if (c < 0) { if (tid == 0) S.g.err = c == -2 ? JOB_ERR_QUERY_LEN : JOB_ERR_PLANE_CAP; c = 0; }
                 cells += c;
                 __syncthreads();

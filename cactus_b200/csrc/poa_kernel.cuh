@@ -16,6 +16,17 @@ struct SlotLayout {
     int64_t o_row_off, o_row_info, o_cigar, o_fc;
 };
 
+// dynamic shared memory per CTA of each CTA-size class, sized so that the class's CTAs per SM still fit: the topological sort's
+// scratch between sweeps, and during a sweep the ring of its last two rows where two rows fit (poa_kernel.cu: dp_sweep)
+HD constexpr int poa_scratch_bytes(int T) {
+    return T == 32 ? 10 * 1024 : T == 64 ? 24 * 1024 : T == 128 ? 40 * 1024 : T == 256 ? 96 * 1024 : 200 * 1024;
+}
+// bytes of the sweep's two-row ring (two rows of T threads x TB ints), 0 for a class whose scratch cannot hold it. The kernel
+// decides at compile time whether a class has a ring, so its launches never get less dynamic shared memory than this
+HD constexpr int poa_ring_bytes(int T) {
+    return 2 * T * TB * (int)sizeof(int) <= poa_scratch_bytes(T) ? 2 * T * TB * (int)sizeof(int) : 0;
+}
+
 enum { PH_DP = 0, PH_BACKTRACK = 1, PH_FUSE = 2, PH_TOPO = 3, PH_MSA = 4, PH_TOTAL = 5, PH_N = 8 };
 
 struct BatchArgs {
