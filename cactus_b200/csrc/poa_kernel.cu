@@ -19,9 +19,9 @@
 //     the CTA's dynamic shared memory, where the class's scratch holds two rows; older ones from the planes in global memory
 //     (L2), one 16-byte chunk per thread and instruction, a warp's chunk 512 contiguous bytes;
 //   * the max-plus recurrence of the two insertion states F1/F2 along the row is turned into a plain prefix
-//     maximum by the substitution A[k] = H'[k] - oe + (k+1)*e  =>  F[j] = max_{k<j} A[k] - j*e: 16 serial cells per
-//     thread, a warp shuffle scan over the 32 thread aggregates, a redux over the warp aggregates staged in
-//     shared memory;
+//     maximum by the substitution A[k] = H'[k] - oe + (k+1)*e  =>  F[j] = max_{k<j} A[k] - j*e across threads: a warp
+//     shuffle scan over the 32 thread aggregates, a redux over the warp aggregates staged in shared memory. Within a
+//     thread's 16 cells the recurrence itself runs, one add-max per cell and plane (row_pass1, row_pass2);
 //   * per cell the sweep writes 8 bytes for the traceback and for later rows -- H (int32) and the two E values as 16-bit
 //     distances below H; F1 / F2 are not stored, the traceback recomputes the few row prefixes it needs
 //     (poa_types.h: DpState) -- in a chunk-major layout where every 128-bit warp store writes 512 contiguous bytes:
@@ -42,7 +42,9 @@ namespace barb200 {
 struct KShared {
     Graph g; RowTables rt; DpState d;
     int job, msa_len_s, abort_s;
-    int smat[5 * 8];       // [graph base][query code 0..4, 5 = "no base": column 0 / beyond the query -> 0]
+    // [graph base][query code 0..4, 5 = "no base": column 0 / beyond the query -> 0]. 256-byte aligned: the sweep forms an
+    // entry's shared-memory address by replacing the low byte of the table's with the byte offset 32 * base + 4 * code
+    __align__(256) int smat[5 * 8];
     int wF[2][2][32];      // [row parity][plane F1/F2][warp] block scan staging
     int wM[2][4][32];      // [row parity][max, leftmost, rightmost, H of the warp's last column][warp]
     RowRec rec[2];         // [row parity] the sweep's row record, fetched one row ahead
@@ -72,9 +74,13 @@ __device__ __forceinline__ int lds1(unsigned a) {
     asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
     return v;
 }
-// the value of v, opaque to the compiler: what is computed from it in the row loop stays there. The 16 per-column gap offsets
-// j*e of each plane, hoisted out of the loop, hold 32 registers across it and are spilled and reloaded in every row
-__device__ __forceinline__ int opaque(int v) { asm volatile("" : "+r"(v)); return v; }
+// a load from a table in shared memory that does not change while the sweep runs: not volatile, so that the compiler can
+// schedule the loads of a row's cells freely
+__device__ __forceinline__ int lds_const(unsigned a) {
+    int v;
+    asm("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a));
+    return v;
+}
 __device__ __forceinline__ int max3(int a, int b, int c) { return max(max(a, b), c); }
 // 16-byte global -> shared copy that bypasses the registers (completes at cp_async_wait_all)
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
@@ -90,23 +96,31 @@ __device__ __forceinline__ void store_pad(int *tp, int64_t cs, int NEG) {
 
 
 // ---- the two per-thread passes over a row's 16 cells, in a branch-free form -------------------------------------
-// "A space" of the F scans: A1'[k] = H'[k] + k*e1 (the constant -o1 is applied when F is read back), so
-// F1[j] = max_{k<j} A1'[k] - o1 - j*e1 and the scan identity is inf_min + beg*e1 + o1. MASKED = some of the thread's
-// columns lie outside [beg, end] (they must come out as exactly inf_min).
+// The block scan of the F states runs in "A space": A1'[k] = H'[k] + k*e1 (the constant -o1 is applied when F is read back),
+// so F1[j] = max_{k<j} A1'[k] - o1 - j*e1 and the scan identity is inf_min + beg*e1 + o1. Within a thread neither pass forms
+// the per-column offsets k*e: pass 1 folds its cells' A values right to left (Horner), pass 2 runs the F recurrence itself.
+// MASKED = some of the thread's columns lie outside [beg, end] (they must come out as exactly inf_min).
+//
+// mbase: shared-memory address of smat (256-byte aligned, so its low byte is 0); qo: byte k of word c is
+// 32 * (the row's graph base) + 4 * (query code of my column 4c + k), the low byte of that column's entry address
 template <bool MASKED>
-__device__ __forceinline__ void row_pass1(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], const int *mrow, const uint32_t (&qc)[2],
-                                          int j0, int beg, int end, int NEG, int je1, int je2, int e1, int e2, int &agg1, int &agg2) {
+__device__ __forceinline__ void row_pass1(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], unsigned mbase, const uint32_t (&qo)[4],
+                                          int j0, int beg, int end, int NEG, int e1, int e2, int &agg1, int &agg2) {
 #pragma unroll
     for (int e = 0; e < CPT; ++e) {
-        const int s = mrow[(qc[e >> 3] >> ((e & 7) * 4)) & 7];
+        const int s = lds_const(__byte_perm(qo[e >> 2], mbase, 0x7650 | (e & 3)));   // the entry's address, one PRMT
         int h = __vimax3_s32(H[e] + s, E1[e], E2[e]);                    // H' = max(M + s, E1, E2), :1033,1050
         if (MASKED) {
             const bool inb = (unsigned)(j0 + e - beg) <= (unsigned)(end - beg);
             h = inb ? h : NEG; E1[e] = inb ? E1[e] : NEG; E2[e] = inb ? E2[e] : NEG;
         }
         H[e] = h;
-        agg1 = __viaddmax_s32(h, je1 + e * e1, agg1); agg2 = __viaddmax_s32(h, je2 + e * e2, agg2);
     }
+    // a = max_k H'[k] + k*e over my cells, folded right to left: a <- max(a + e, H'[k]); then the thread's aggregate in A space
+    int a1 = H[CPT - 1], a2 = H[CPT - 1];
+#pragma unroll
+    for (int e = CPT - 2; e >= 0; --e) { a1 = __viaddmax_s32(a1, e1, H[e]); a2 = __viaddmax_s32(a2, e2, H[e]); }
+    agg1 = max(agg1, a1 + j0 * e1); agg2 = max(agg2, a2 + j0 * e2);
 }
 
 // folds chunk oc of a predecessor row (4 H values, 4 D codes) into my columns' candidates: H[e+1] <- the M input H_pred[e],
@@ -127,21 +141,24 @@ __device__ __forceinline__ void pred_chunk(int (&H)[CPT], int (&E1)[CPT], int (&
 // MODE 0: all of the warp's active columns are inside the band; 1: some lie left (or left and right) of it -- every value
 // of an outside cell is forced to inf_min; 2: some lie right of it only -- nothing in the band depends on those cells
 // and the traceback never reads the F planes outside the band, so only H / E1 / E2 are forced (they feed later rows).
-// RING_NT: threads per CTA if the row also goes to the shared-memory ring (rs: address of my chunk 0 of the slot), else 0
+// RING_NT: threads per CTA if the row also goes to the shared-memory ring (rs: address of my chunk 0 of the slot), else 0.
+// F1 / F2: the insertion states of my first column, P - o - j0*e from the block scan's exclusive prefix P. From there the
+// recurrence F[j+1] = max(F[j] - e, H'[j] - oe) gives, integer for integer, the A-space value max_{k<=j} A'[k] - o - (j+1)*e
+// (both sides are max(P, max_{k<=j} H'[k] + k*e) - o - (j+1)*e), so the pass forms no F value the A-space scan does not; the
+// other terms, F - e and H' - oe, lie at most oe below an F value or an H' value, as h - oe of the E update does. The int32 range
+// argument of the A-space sweep (DESIGN section 7: nothing above H' + (j+1)*e) therefore covers this pass unchanged.
 template <int MODE, int RING_NT>
-__device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], int P1, int P2, int j0, int beg, int end, int NEG,
-                                          int je1, int je2, int e1, int e2, int o1, int o2, int *tp, int64_t cs, unsigned rs, int &tmax) {
-    const int oe1 = o1 + e1, oe2 = o2 + e2;
+__device__ __forceinline__ void row_pass2(int (&H)[CPT], int (&E1)[CPT], int (&E2)[CPT], int F1, int F2, int j0, int beg, int end, int NEG,
+                                          int e1, int e2, int oe1, int oe2, int *tp, int64_t cs, unsigned rs, int &tmax) {
     // one H chunk and one D chunk per 4 cells (tp: the thread's chunk 0, cs: ints between chunks; poa_types.h: DpState)
 #pragma unroll
     for (int oc = 0; oc < CPT / CHUNK; ++oc) {
         int dd[CHUNK];
 #pragma unroll
         for (int u = 0; u < CHUNK; ++u) {
-            const int e = oc * CHUNK + u, u1 = je1 + e * e1, u2 = je2 + e * e2;
-            const int f1 = P1 - o1 - u1, f2 = P2 - o2 - u2;                // F[j] = max_{k<j} A'[k] - o - j*e (used, not stored)
-            P1 = __viaddmax_s32(H[e], u1, P1); P2 = __viaddmax_s32(H[e], u2, P2);
-            int h = __vimax3_s32(H[e], f1, f2);                            // :1067
+            const int e = oc * CHUNK + u, hp = H[e];                       // H' of the cell, before F
+            int h = __vimax3_s32(hp, F1, F2);                              // :1067 (F used, not stored)
+            F1 = __viaddmax_s32(F1, -e1, hp - oe1); F2 = __viaddmax_s32(F2, -e2, hp - oe2);   // F of the next column
             int x1 = __viaddmax_s32(E1[e], -e1, h - oe1);                  // E for the next rows, :1070-1071
             int x2 = __viaddmax_s32(E2[e], -e2, h - oe2);
             if (MODE == 1) {
@@ -190,7 +207,7 @@ __device__ __forceinline__ void row_argmax(const int (&H)[CPT], int v, int j0, i
 // r - 2 wrote their slots before barriers row r has already passed.
 // ---------------------------------------------------------------------------------------------------------
 template <int NT>
-__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L, uint2 *qsm, unsigned ring) {
+__device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__restrict__ qg, int L, uint4 *qsm, unsigned ring) {
     constexpr int RING_NT = poa_ring_bytes(NT) ? NT : 0;                        // a compile-time property of the class
     constexpr unsigned SLOT = NT * TB * sizeof(int), RCS = NT * 16;              // ring bytes per slot, between chunks
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = NT >> 5;
@@ -212,18 +229,20 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
     static_assert(CPT == 16, "shifts below assume 16 columns per thread");
     const int j0 = tid * CPT;
 
-    // query codes of my 16 columns, 4 bits each (column j scores against q_j = qg[j-1]; column 0 and columns past the
-    // query score 0, abpoa_align_simd.c:536)
-    uint32_t qc[2] = {0u, 0u};
+    // query codes of my 16 columns as byte offsets 4 * code into a row of smat, one byte each (column j scores against
+    // q_j = qg[j-1]; column 0 and columns past the query score 0, abpoa_align_simd.c:536). A row adds 32 * base to every
+    // byte: 32 * 4 + 4 * 5 < 256, no byte carries into the next
+    uint32_t qo[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
     for (int e = 0; e < CPT; ++e) {
         const int j = j0 + e;
         const uint32_t c = (j >= 1 && j <= L) ? qg[j - 1] : 5u;
-        qc[e >> 3] |= c << ((e & 7) * 4);
+        qo[e >> 2] |= (4u * c) << ((e & 3) * 8);
     }
-    // they are read back from shared memory in every row (only by this thread): kept in registers across the row loop, they let
-    // the compiler hoist 16 per-column table offsets out of it, which then spill
-    qsm[tid] = make_uint2(qc[0], qc[1]);
+    // they are read back from shared memory in every row (only by this thread, one 128-bit load): codes kept in registers across
+    // the row loop let the compiler hoist 16 per-column table offsets out of it, which then spilled
+    qsm[tid] = make_uint4(qo[0], qo[1], qo[2], qo[3]);
+    const unsigned smat_s = (unsigned)__cvta_generic_to_shared(S.smat);           // low byte 0 (256-byte aligned)
 
     int H[CPT], E1[CPT], E2[CPT];          // the previous row's values of my columns (valid iff prev_active)
     bool prev_active;
@@ -306,7 +325,7 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
         // masking is decided per WARP (no divergent double execution): 0 = all active threads inside the band,
         // 1 = some columns left of the band, 2 = some columns right of it only
         const int wmode = __any_sync(FULL, active && j0 < beg) ? 1 : __any_sync(FULL, active && j0 + CPT - 1 > end) ? 2 : 0;
-        const int *mrow = S.smat + 8 * b;
+        const uint32_t qadd = 0x01010101u * (32u * b);                  // table row b: 32 * b added to every byte offset
 
         // H of the column left of my first one, previous row
         int hl = __shfl_up_sync(FULL, prev_active ? H[CPT - 1] : NEG, 1);
@@ -358,11 +377,10 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
                 // H[16*tid - 1]: the last H (chunk 3) of the left neighbour's block
                 if (ptt >= 1 && ptt <= pnT) H[0] = max(H[0], __ldcg(Hp - CHUNK + (CPT / CHUNK - 1) * pcs + CHUNK - 1));
             }
-            const uint2 q2 = qsm[tid];
-            const uint32_t qr[2] = {q2.x, q2.y};
-            const int pe1 = opaque(e1), pe2 = opaque(e2);
-            if (wmode != 1) row_pass1<false>(H, E1, E2, mrow, qr, j0, beg, end, NEG, j0 * pe1, j0 * pe2, pe1, pe2, agg1, agg2);
-            else row_pass1<true>(H, E1, E2, mrow, qr, j0, beg, end, NEG, j0 * pe1, j0 * pe2, pe1, pe2, agg1, agg2);
+            const uint4 q4 = qsm[tid];
+            const uint32_t qo[4] = {q4.x + qadd, q4.y + qadd, q4.z + qadd, q4.w + qadd};
+            if (wmode != 1) row_pass1<false>(H, E1, E2, smat_s, qo, j0, beg, end, NEG, e1, e2, agg1, agg2);
+            else row_pass1<true>(H, E1, E2, smat_s, qo, j0, beg, end, NEG, e1, e2, agg1, agg2);
         }
         // ---- exclusive prefix maximum over the row: warp shuffle scan + redux over warp aggregates ----
         int inc1 = agg1, inc2 = agg2;
@@ -390,10 +408,10 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
             const int64_t cs = chunk_index(nTs, 0, 1);
             const unsigned rs = my_ring + par * SLOT;
             if (active) {
-                const int pe1 = opaque(e1), pe2 = opaque(e2), je1 = j0 * pe1, je2 = j0 * pe2;
-                if (wmode == 0) row_pass2<0, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
-                else if (wmode == 2) row_pass2<2, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
-                else row_pass2<1, RING_NT>(H, E1, E2, P1, P2, j0, beg, end, NEG, je1, je2, pe1, pe2, P.o1, P.o2, tp, cs, rs, tmax);
+                const int F1 = P1 - P.o1 - j0 * e1, F2 = P2 - P.o2 - j0 * e2;   // F of my first column
+                if (wmode == 0) row_pass2<0, RING_NT>(H, E1, E2, F1, F2, j0, beg, end, NEG, e1, e2, oe1, oe2, tp, cs, rs, tmax);
+                else if (wmode == 2) row_pass2<2, RING_NT>(H, E1, E2, F1, F2, j0, beg, end, NEG, e1, e2, oe1, oe2, tp, cs, rs, tmax);
+                else row_pass2<1, RING_NT>(H, E1, E2, F1, F2, j0, beg, end, NEG, e1, e2, oe1, oe2, tp, cs, rs, tmax);
             } else if ((unsigned)tts < (unsigned)nTs) store_pad(tp, cs, NEG);
         }
         // ---- left/right-most argmax of H over the band (simd_abpoa_max_in_row, :1107-1119) ----
@@ -453,7 +471,7 @@ template <int NT>
 __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
     extern __shared__ __align__(16) unsigned char dyn_smem[];    // scratch of the topological sort (poa_cta.cuh), the sweep's row ring
     __shared__ KShared S;
-    __shared__ uint2 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
+    __shared__ uint4 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
     const int tid = threadIdx.x;
     int *ws = &S.wF[0][0][0];
     if (tid == 0) carve(S, A, blockIdx.x);
