@@ -204,18 +204,7 @@ void *pinned_take(barb200_ctx *ctx, size_t bytes, size_t *got) { return ::pinned
 void pinned_give(barb200_ctx *ctx, void *p, size_t bytes) { ::pinned_give(*ctx->devs[0], p, bytes); }
 }  // namespace barb200
 
-extern "C" void barb200_params_default(barb200_params *p) {
-    static const int mat[25] = {91, -114, -61, -123, -100, -114, 100, -125, -61, -100, -61, -125, 100, -114, -100,
-                                -123, -61, -114, 91, -100, -100, -100, -100, -100, 100};
-    memset(p, 0, sizeof(*p));
-    memcpy(p->mat, mat, sizeof(mat));
-    p->gap_open1 = 400; p->gap_ext1 = 30; p->gap_open2 = 1200; p->gap_ext2 = 1;
-    p->wb = 1000; p->wf = 0.1f;
-    p->k = 15; p->w = 5; p->min_w = 500;
-    p->progressive_poa = 1; p->disable_seeding = 1;
-    p->device = 0; p->threads_per_block = 0; p->ctas_per_sm = 0; p->mem_fraction = 0.0; p->host_threads = 0;
-    p->collect_phase_clocks = 0; p->n_devices = 0; p->lanes = 0;
-}
+extern "C" void barb200_params_default(barb200_params *p) { params_default(p); }
 
 static void fail(char *errbuf, int n, const std::string &m) { if (errbuf && n > 0) { snprintf(errbuf, n, "%s", m.c_str()); } }
 
@@ -252,14 +241,7 @@ extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *errbuf, in
     ctx->p = *p;
     ctx->lanes_per_device = p->lanes > 0 ? std::min(p->lanes, 2) : 2;
     if (getenv("BARB200_LANES")) ctx->lanes_per_device = std::max(1, std::min(2, atoi(getenv("BARB200_LANES"))));
-    PoaParams &P = ctx->P;
-    memcpy(P.mat, p->mat, sizeof(P.mat));
-    P.o1 = p->gap_open1; P.e1 = p->gap_ext1; P.o2 = p->gap_open2; P.e2 = p->gap_ext2; P.wb = p->wb; P.wf = p->wf;
-    P.max_mat = 0; P.min_mis = 0;
-    for (int i = 0; i < 25; ++i) { P.max_mat = std::max(P.max_mat, P.mat[i]); P.min_mis = std::max(P.min_mis, -P.mat[i]); }
-    // the reference's int32 minus infinity, abpoa_align_simd.c:1299
-    const int oe1 = P.o1 + P.e1, oe2 = P.o2 + P.e2;
-    P.inf_min = std::max(std::max(INT32_MIN + P.min_mis, INT32_MIN + oe1), INT32_MIN + oe2) + 512 * std::max(P.e1, P.e2);
+    ctx->P = poa_params(p->mat, p->gap_open1, p->gap_ext1, p->gap_open2, p->gap_ext2, p->wb, p->wf);
     ctx->hp = HostParams{p->k, p->w, p->min_w, p->progressive_poa};
     int lane_index = 0;
     for (int ord : ords) {
@@ -353,8 +335,6 @@ struct Bucket {
     SlotLayout lay; int slots = 0;
     size_t slot_off = 0; int64_t plane_off = 0; size_t clk_off = 0;   // offsets into the lane's arena (bytes / ints / entries)
 };
-
-static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 static int class_of_len(barb200_ctx *ctx, int64_t max_len) {
     for (int i = 0; i < kNumKernels; ++i) if ((int64_t)kKernels[i].T * CPT >= max_len + 1 && kKernels[i].T >= ctx->p.threads_per_block) return i;
@@ -468,35 +448,12 @@ static int plan_stage(barb200_stage *st) {
     Device &D = dev_of_lane(ctx, st->lane);
     Lane &LN = lane_of(ctx, st->lane);
     for (Bucket &B : st->buckets) {
-        int64_t max_nodes = 4, max_edges = 4, max_len = 1, max_k = 1, plane_need = 0;
+        SlotNeeds need;
         for (int64_t j = B.job_base; j < B.job_base + B.n_jobs; ++j) {
             const TableJob &J = st->tab->jobs[st->perm[j]];
-            const int64_t sum = J.sum_len, ml = J.max_len, K = J.n_seq;
-            max_nodes = std::max(max_nodes, sum + 2); max_edges = std::max(max_edges, sum + K); max_len = std::max(max_len, ml);
-            max_k = std::max(max_k, K);
-            plane_need = std::max(plane_need, plane_ints_for_job(ctx->P.wb, ctx->P.wf, K, sum, ml, st->grow, st->worst_case));
+            need.add_job(J.n_seq, J.sum_len, J.max_len, plane_ints_for_job(ctx->P.wb, ctx->P.wf, J.n_seq, J.sum_len, J.max_len, st->grow, st->worst_case));
         }
-        SlotLayout &Y = B.lay;
-        memset(&Y, 0, sizeof(Y));
-        Y.node_cap = (int)max_nodes; Y.in_pool = (int)(4 * max_edges + 64); Y.out_pool = Y.in_pool;
-        Y.W = (int)(1 + ((max_k - 1) >> 6)); Y.cigar_cap = (int)(max_len + max_nodes + 16);
-        Y.plane_cap = align_up(plane_need, 8);
-        int64_t o = 0;
-        auto take = [&](int64_t bytes) { int64_t r = o; o = align_up(o + bytes, 16); return r; };
-        const int64_t N = Y.node_cap;
-        Y.o_base = take(N); Y.o_aln_n = take(N); Y.o_aln_id = take(N * 16);
-        Y.o_in_off = take(N * 4); Y.o_in_n = take(N * 4); Y.o_in_cap = take(N * 4);
-        Y.o_out_off = take(N * 4); Y.o_out_n = take(N * 4); Y.o_out_cap = take(N * 4);
-        Y.o_in_id = take((int64_t)Y.in_pool * 4); Y.o_in_w = take((int64_t)Y.in_pool * 4);
-        Y.o_out_id = take((int64_t)Y.out_pool * 4); Y.o_out_w = take((int64_t)Y.out_pool * 4);
-        Y.o_out_rid = take((int64_t)Y.out_pool * 8 * Y.W);
-        Y.o_index_to_node = take(N * 4); Y.o_node_to_index = take(N * 4); Y.o_remain = take(N * 4); Y.o_msa_rank = take(N * 4);
-        Y.o_tmp0 = take(N * 4); Y.o_tmp1 = take(N * 4);
-        Y.o_row_rec = take(N * 16); Y.o_pre_row = take((int64_t)Y.in_pool * 4);
-        Y.o_row_off = take(N * 8); Y.o_row_info = take(N * 16);
-        Y.o_cigar = take((int64_t)Y.cigar_cap * 8);
-        Y.fc_cap = (int)(max_len + 2); Y.o_fc = take((int64_t)Y.fc_cap * 8);
-        Y.slot_bytes = align_up(o, 256);
+        B.lay = plan_slot(need);
         B.T = kKernels[B.cls].T; B.dyn_smem = kKernels[B.cls].scratch;
         if (getenv("BARB200_SCRATCH_KB")) B.dyn_smem = (size_t)atoi(getenv("BARB200_SCRATCH_KB")) * 1024;   // tuning aid
         // never below the sweep's ring, which the kernel uses without a run-time check (the topological sort and the MSA ranking
@@ -618,39 +575,24 @@ static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTabl
     const int64_t ns = st->n_seqs = lo;
     st->msa_bytes = msa_off;
     if (n_jobs == 0) { *out = st.release(); return BARB200_OK; }
-    // device buffers (one cached block) + upload on the lane's copy stream, so that it overlaps a running kernel
-    size_t off = 0;
-    auto sub = [&](size_t bytes) { size_t r = off; off = (off + std::max<size_t>(bytes, 16) + 255) & ~(size_t)255; return r; };
-    // K0's scratch: one slot per resident guide-tree CTA, sized from the stage's largest job (keys: ~2 / (w + 1) per base; ties in
-    // repeats can push up to 2 w per base -- capacity misses are retried like the planes')
+    // K0's scratch: one slot per resident guide-tree CTA, sized from the stage's largest job
     GuideTreeArgs &GA = st->gt;
     memset(&GA, 0, sizeof(GA));
-    {
-        int64_t key_need = 64, gx_need = 8, mk = 1;
-        for (int64_t c : st->perm) {
-            const TableJob &J = T.jobs[c];
-            if (!(J.progressive && J.n_seq > 2)) continue;
-            const int64_t sum = J.sum_len, worst = 2 * (int64_t)ctx->p.w * sum + J.n_seq;
-            key_need = std::max(key_need, worst_case ? worst : std::min<int64_t>(worst, (int64_t)(grow * (double)(sum / 2 + 64))));
-            gx_need = std::max(gx_need, sum); mk = std::max<int64_t>(mk, J.n_seq);
-        }
-        int64_t kc = 64; while (kc < key_need) kc <<= 1;            // the sort pads to a power of two
-        int64_t o = 0;
-        auto take = [&](int64_t bytes) { int64_t r = o; o = align_up(o + bytes, 16); return r; };
-        GA.key_cap = (int)kc;
-        GA.o_keys = take(kc * 8); GA.o_gx = take(gx_need * 8); GA.o_hit = take(mk * (mk + 1) / 2 * 4); GA.o_jac = take(mk * (mk - 1) / 2 * 8 + 8); GA.o_score = take(mk * 8);
-        GA.slot_bytes = align_up(o, 256);
-        st->gt_ctas = (int)std::min<int64_t>(std::min<int64_t>(n_jobs, (int64_t)4 * D.sm_count), std::max<int64_t>(1, ((int64_t)2 << 30) / GA.slot_bytes));
-    }
-    const size_t o_seqs = d_seqs ? 0 : sub(T.n_bases), o_lens = sub(ns * 4), o_soff = sub(ns * 8), o_desc = sub(n_jobs * sizeof(JobDesc)),
-                 o_msa = sub(st->msa_bytes), o_msa_len = sub(n_jobs * 4), o_status = sub(n_jobs * 4), o_cells = sub(n_jobs * 8), o_next = sub(4 * (kNumKernels + 1)),
-                 o_order = sub(ns * 4), o_gts = sub(n_jobs * 4), o_gtscr = sub((size_t)GA.slot_bytes * st->gt_ctas);
-    st->d_block_bytes = off;
+    GtNeeds gt_need;
+    for (int64_t c : st->perm) gt_need.add_job(T.jobs[c].progressive, T.jobs[c].n_seq, T.jobs[c].sum_len, ctx->p.w, grow, worst_case);
+    GA.lay = plan_gt_scratch(gt_need);
+    st->gt_ctas = (int)std::min<int64_t>(std::min<int64_t>(n_jobs, (int64_t)4 * D.sm_count), std::max<int64_t>(1, ((int64_t)2 << 30) / GA.lay.slot_bytes));
+    // device buffers (one cached block) + upload on the lane's copy stream, so that it overlaps a running kernel
+    BumpOffsets sub{256};
+    const int64_t o_seqs = d_seqs ? 0 : sub.take(T.n_bases), o_lens = sub.take(ns * 4), o_soff = sub.take(ns * 8), o_desc = sub.take(n_jobs * sizeof(JobDesc)),
+                  o_msa = sub.take(st->msa_bytes), o_msa_len = sub.take(n_jobs * 4), o_status = sub.take(n_jobs * 4), o_cells = sub.take(n_jobs * 8),
+                  o_next = sub.take(4 * (kNumKernels + 1)), o_order = sub.take(ns * 4), o_gts = sub.take(n_jobs * 4), o_gtscr = sub.take(GA.lay.slot_bytes * st->gt_ctas);
+    st->d_block_bytes = (size_t)sub.end;
     const double tb2 = now_ms();
     int rc = plan_stage(st.get());
     if (rc) return rc;
     const double tb3 = now_ms();
-    cudaError_t e = dev_alloc(D, &st->d_block, off);
+    cudaError_t e = dev_alloc(D, &st->d_block, st->d_block_bytes);
     if (e != cudaSuccess) {
         cudaGetLastError(); set_error(ctx, std::string("cudaMalloc(stage) failed: ") + cudaGetErrorString(e));
         st->d_block = nullptr; return BARB200_ENOMEM;

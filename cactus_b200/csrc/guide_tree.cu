@@ -13,11 +13,8 @@ __global__ void __launch_bounds__(kGuideTreeThreads, 4) guide_tree_kernel(const 
     __shared__ int s_job, s_n_keys;
     __shared__ double ws_v[33];
     __shared__ long long ws_i[33];
-    uint8_t *const sb = A.scratch + (int64_t)blockIdx.x * A.slot_bytes;
-    GtScratch G;
-    G.keys = reinterpret_cast<uint64_t *>(sb + A.o_keys); G.key_cap = A.key_cap; G.gx = reinterpret_cast<uint64_t *>(sb + A.o_gx);
-    G.hit = reinterpret_cast<int *>(sb + A.o_hit); G.jac = reinterpret_cast<double *>(sb + A.o_jac); G.score = reinterpret_cast<double *>(sb + A.o_score);
-    G.n_keys = &s_n_keys; G.red_i = nullptr; G.red_v = nullptr; G.tile = tile; G.tile_cap = kGuideTreeTileKeys;
+    GtScratch G = gt_views(A.lay, A.scratch + (int64_t)blockIdx.x * A.lay.slot_bytes);
+    G.n_keys = &s_n_keys; G.tile = tile; G.tile_cap = kGuideTreeTileKeys;
     const GuideTreeParams GP{A.k, A.w};
     while (true) {
         if (threadIdx.x == 0) s_job = atomicAdd(A.next_job, 1);

@@ -16,6 +16,7 @@
 //      reads placed so far, accumulated in placement order exactly like the reference's inner loop, first maximum wins.
 // The same source compiles for the host (tests/hosttest), where the T threads of every phase run one after the other.
 #pragma once
+#include <math.h>
 #include <stdint.h>
 #include "poa_types.h"
 
@@ -219,7 +220,7 @@ HD int cta_guide_tree(const GuideTreeParams &P, int progressive, int n, SeqFn se
             GT_THREADS(tid, T) {
                 for (int t0 = tid; t0 < (n2 >> 1); t0 += 4 * T) {
                     uint64_t a[4], b[4]; int lo[4];
-#if defined(__CUDACC__)
+#if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
                     for (int u = 0; u < 4; ++u) {
@@ -227,7 +228,7 @@ HD int cta_guide_tree(const GuideTreeParams &P, int progressive, int n, SeqFn se
                         lo[u] = t < (n2 >> 1) ? ((t / stride) * (stride << 1)) + (t % stride) : -1;
                         if (lo[u] >= 0) { a[u] = G.keys[lo[u]]; b[u] = G.keys[lo[u] + stride]; }
                     }
-#if defined(__CUDACC__)
+#if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
                     for (int u = 0; u < 4; ++u) if (lo[u] >= 0) {

@@ -1,11 +1,24 @@
 // host_api.h -- internal C++ interfaces between the host-side translation units of libbarb200.
 #pragma once
 #include <stdint.h>
+#include <string.h>
 #include <string>
 #include <vector>
 #include "../../include/barb200.h"
 
 namespace barb200 {
+
+// barb200_params_default: Cactus' defaults, every field not set here 0
+inline void params_default(barb200_params *p) {
+    static const int mat[25] = {91, -114, -61, -123, -100, -114, 100, -125, -61, -100, -61, -125, 100, -114, -100,
+                                -123, -61, -114, 91, -100, -100, -100, -100, -100, 100};
+    memset(p, 0, sizeof(*p));
+    memcpy(p->mat, mat, sizeof(mat));
+    p->gap_open1 = 400; p->gap_ext1 = 30; p->gap_open2 = 1200; p->gap_ext2 = 1;
+    p->wb = 1000; p->wf = 0.1f;
+    p->k = 15; p->w = 5; p->min_w = 500;
+    p->progressive_poa = 1; p->disable_seeding = 1;
+}
 
 struct HostParams {
     int k, w, min_w, progressive_poa;

@@ -445,26 +445,6 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
     return cells;
 }
 
-__device__ __forceinline__ void carve(KShared &S, const BatchArgs &A, int slot) {
-    const SlotLayout &Y = A.lay;
-    uint8_t *b = A.slots + (int64_t)slot * Y.slot_bytes;
-    Graph &g = S.g; RowTables &rt = S.rt; DpState &d = S.d;
-    g.node_cap = Y.node_cap; g.in_pool = Y.in_pool; g.out_pool = Y.out_pool;
-    g.base = b + Y.o_base; g.aln_n = b + Y.o_aln_n; g.aln_id = (int *)(b + Y.o_aln_id);
-    g.in_off = (int *)(b + Y.o_in_off); g.in_n = (int *)(b + Y.o_in_n); g.in_cap = (int *)(b + Y.o_in_cap);
-    g.out_off = (int *)(b + Y.o_out_off); g.out_n = (int *)(b + Y.o_out_n); g.out_cap = (int *)(b + Y.o_out_cap);
-    g.in_id = (int *)(b + Y.o_in_id); g.in_w = (int *)(b + Y.o_in_w);
-    g.out_id = (int *)(b + Y.o_out_id); g.out_w = (int *)(b + Y.o_out_w); g.out_rid = (uint64_t *)(b + Y.o_out_rid);
-    g.index_to_node = (int *)(b + Y.o_index_to_node); g.node_to_index = (int *)(b + Y.o_node_to_index);
-    g.remain = (int *)(b + Y.o_remain); g.msa_rank = (int *)(b + Y.o_msa_rank);
-    g.tmp0 = (int *)(b + Y.o_tmp0); g.tmp1 = (int *)(b + Y.o_tmp1);
-    rt.rec = (RowRec *)(b + Y.o_row_rec); rt.pre_row = (int *)(b + Y.o_pre_row);
-    d.planes = A.planes + (int64_t)slot * Y.plane_cap; d.plane_cap = Y.plane_cap;
-    d.row_off = (int64_t *)(b + Y.o_row_off); d.info = (RowInfo *)(b + Y.o_row_info);
-    d.cigar = (uint64_t *)(b + Y.o_cigar); d.cigar_cap = Y.cigar_cap; d.n_cigar = 0;
-    d.fc = (int *)(b + Y.o_fc); d.fc_cap = Y.fc_cap; d.fc_row = -1; d.fc_hi = -1;
-}
-
 #define PHASE_TICK(ph) do { if (A.phase_clk && threadIdx.x == 0) { unsigned long long _n = clock64(); A.phase_clk[(size_t)blockIdx.x * PH_N + (ph)] += _n - t_last; t_last = _n; } } while (0)
 
 template <int NT>
@@ -474,7 +454,9 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
     __shared__ uint4 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
     const int tid = threadIdx.x;
     int *ws = &S.wF[0][0][0];
-    if (tid == 0) carve(S, A, blockIdx.x);
+    // the slot index as an int: addresses formed exactly as dp_sweep forms its own (from the unsigned blockIdx.x) would be
+    // computed once here and kept live through the whole kernel, which spills t64 .. t256
+    if (tid == 0) { const int slot = blockIdx.x; slot_views(A.lay, A.slots + (int64_t)slot * A.lay.slot_bytes, A.planes + (int64_t)slot * A.lay.plane_cap, S.g, S.rt, S.d); }
     for (int k = tid; k < 40; k += blockDim.x) S.smat[k] = (k & 7) < 5 ? A.P.mat[(k >> 3) * 5 + (k & 7)] : 0;
     unsigned long long t_last = A.phase_clk ? clock64() : 0ULL, t_start = t_last;
     __syncthreads();

@@ -1,20 +1,9 @@
 // poa_kernel.cuh -- device-side arguments of the fused batched POA kernel (see poa_kernel.cu).
 #pragma once
 #include "poa_types.h"
+#include "slot_plan.h"
 
 namespace barb200 {
-
-// Byte offsets of every per-slot array from the slot base (computed once per batch on the host).
-struct SlotLayout {
-    int64_t slot_bytes;
-    int node_cap, in_pool, out_pool, W, cigar_cap, fc_cap;
-    int64_t plane_cap;   // ints per slot
-    int64_t o_base, o_aln_n, o_aln_id, o_in_off, o_in_n, o_in_cap, o_out_off, o_out_n, o_out_cap;
-    int64_t o_in_id, o_in_w, o_out_id, o_out_w, o_out_rid;
-    int64_t o_index_to_node, o_node_to_index, o_remain, o_msa_rank, o_tmp0, o_tmp1;
-    int64_t o_row_rec, o_pre_row;
-    int64_t o_row_off, o_row_info, o_cigar, o_fc;
-};
 
 // dynamic shared memory per CTA of each CTA-size class, sized so that the class's CTAs per SM still fit: the topological sort's
 // scratch between sweeps, and during a sweep the ring of its last two rows where two rows fit (poa_kernel.cu: dp_sweep)
@@ -55,8 +44,7 @@ struct GuideTreeArgs {
     int *order;                 // out: per sequence slot, indexed like lens
     int *gt_status;             // out: per job, 0 or JOB_ERR_GT_CAP
     int *next_job;              // work counter
-    uint8_t *scratch; int64_t slot_bytes;       // per-CTA scratch
-    int64_t o_keys, o_gx, o_hit, o_jac, o_score; int key_cap;
+    uint8_t *scratch; GtLayout lay;             // per-CTA scratch slots
     int k, w;
 };
 constexpr int kGuideTreeThreads = 256;

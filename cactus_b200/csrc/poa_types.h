@@ -149,4 +149,15 @@ HD int e_encode(int h, int e) { const int d = h - e; return (d >= 0 && d < E_NEG
 HD int imax(int a, int b) { return a > b ? a : b; }
 HD int imin(int a, int b) { return a < b ? a : b; }
 
+// The DP's parameters from the substitution matrix, the two gap pairs and the band, with the fields derived from them
+inline PoaParams poa_params(const int mat[25], int o1, int e1, int o2, int e2, int wb, float wf) {
+    PoaParams P;
+    P.o1 = o1; P.e1 = e1; P.o2 = o2; P.e2 = e2; P.wb = wb; P.wf = wf;
+    P.max_mat = 0; P.min_mis = 0;
+    for (int i = 0; i < 25; ++i) { P.mat[i] = mat[i]; P.max_mat = imax(P.max_mat, mat[i]); P.min_mis = imax(P.min_mis, -mat[i]); }
+    // the reference's int32 minus infinity, abpoa_align_simd.c:1299
+    P.inf_min = imax(imax(INT32_MIN + P.min_mis, INT32_MIN + o1 + e1), INT32_MIN + o2 + e2) + 512 * imax(e1, e2);
+    return P;
+}
+
 }  // namespace barb200

@@ -13,6 +13,7 @@
 #include <math.h>
 #include "../../cactus_b200/csrc/poa_graph.cuh"
 #include "../../cactus_b200/csrc/guide_tree.cuh"
+#include "../../cactus_b200/csrc/slot_plan.h"
 #include "../../cactus_b200/csrc/host_api.h"
 
 using namespace barb200;
@@ -127,45 +128,35 @@ static void incremental_order(Graph &g, const uint8_t *seq, const uint64_t *ciga
     }
 }
 
+// slot memory as the device has it: 256-byte aligned blocks (slot_plan.h)
+struct alignas(256) HtBlock { uint8_t b[256]; };
+
 // same word layout as oracle/ref_harness.c:ref_poa_msa_trace; returns malloc'd words
 extern "C" int64_t *hosttest_poa_msa_trace(const HtParams *hp, int n_seq, const int *lens, const uint8_t *flat, int64_t *n_words, int *status) {
-    PoaParams P; memcpy(P.mat, hp->mat, sizeof(P.mat));
-    P.o1 = hp->o1; P.e1 = hp->e1; P.o2 = hp->o2; P.e2 = hp->e2; P.wb = hp->wb; P.wf = hp->wf; P.max_mat = 0; P.min_mis = 0;
-    for (int i = 0; i < 25; ++i) { P.max_mat = std::max(P.max_mat, P.mat[i]); P.min_mis = std::max(P.min_mis, -P.mat[i]); }
-    P.inf_min = std::max(std::max(INT32_MIN + P.min_mis, INT32_MIN + P.o1 + P.e1), INT32_MIN + P.o2 + P.e2) + 512 * std::max(P.e1, P.e2);
+    const PoaParams P = poa_params(hp->mat, hp->o1, hp->e1, hp->o2, hp->e2, hp->wb, hp->wf);
     std::vector<const uint8_t *> seqs(n_seq); int64_t sum = 0; int maxl = 0;
     for (int i = 0; i < n_seq; ++i) { seqs[i] = flat + sum; sum += lens[i]; maxl = std::max(maxl, lens[i]); }
     std::vector<int> order(n_seq);
-    {   // the product's guide tree (guide_tree.cuh), a block of 64 emulated threads
-        int64_t kc = 64; while (kc < 2 * (int64_t)hp->w * sum + n_seq) kc <<= 1;
-        std::vector<uint64_t> keys((size_t)kc), gx((size_t)sum + 8), tile(256);       // a small tile: the global-stride passes run too
-        std::vector<int> hit((size_t)n_seq * (n_seq + 1) / 2 + 1);
-        std::vector<double> jac((size_t)n_seq * (n_seq - 1) / 2 + 1), score(n_seq);
+    {   // the product's guide tree (guide_tree.cuh) on the product's scratch layout at its worst case, a block of 64 emulated threads
+        GtNeeds need;
+        need.add_job(hp->progressive, n_seq, sum, hp->w, 1.0, true);
+        const GtLayout Y = plan_gt_scratch(need);
+        std::vector<HtBlock> scratch((size_t)Y.slot_bytes / sizeof(HtBlock));
+        std::vector<uint64_t> tile(256);       // a small tile: the global-stride passes run too
         int n_keys = 0; double wsv[33]; long long wsi[33];
-        GtScratch G; G.keys = keys.data(); G.key_cap = (int)kc; G.gx = gx.data(); G.hit = hit.data(); G.jac = jac.data(); G.score = score.data(); G.n_keys = &n_keys; G.red_i = nullptr; G.red_v = nullptr; G.tile = tile.data(); G.tile_cap = (int)tile.size();
+        GtScratch G = gt_views(Y, scratch.data()->b);
+        G.n_keys = &n_keys; G.tile = tile.data(); G.tile_cap = (int)tile.size();
         const GuideTreeParams GP{hp->k, hp->w};
         if (cta_guide_tree(GP, hp->progressive, n_seq, [&](int i) { return seqs[i]; }, lens, order.data(), G, wsv, wsi, 64) != 0) { *status = JOB_ERR_GT_CAP; *n_words = 0; return nullptr; }
     }
-    const int N = (int)sum + 2, EP = (int)(4 * (sum + n_seq) + 64), W = 1 + ((n_seq - 1) >> 6);
+    // the product's slot layout for this one job, its planes at the product's worst case (capped at 2^31 ints)
+    SlotNeeds need;
+    need.add_job(n_seq, sum, maxl, std::min<int64_t>(plane_ints_for_job(P.wb, P.wf, n_seq, sum, maxl, 1.0, true), (int64_t)1 << 31));
+    const SlotLayout Y = plan_slot(need);
+    std::vector<HtBlock> slot((size_t)Y.slot_bytes / sizeof(HtBlock));
+    std::vector<int> planes((size_t)Y.plane_cap);
     Graph g; RowTables rt; DpState d;
-    std::vector<uint8_t> base(N), aln_n(N);
-    std::vector<int> aln_id(4 * N), in_off(N), in_n(N), in_cap(N), out_off(N), out_n(N), out_cap(N), in_id(EP), in_w(EP), out_id(EP), out_w(EP),
-        i2n(N), n2i(N), remain(N), rank(N), t0(N), t1(N), pre_row(EP);
-    std::vector<RowRec> rrec(N); std::vector<RowInfo> rinfo(N);
-    std::vector<uint64_t> rid((size_t)EP * W), cigar(maxl + N + 16);
-    std::vector<int64_t> row_off(N);
-    const int64_t plane_cap = (int64_t)N * (TB / CPT) * (maxl + 2 * CPT);
-    std::vector<int> fcache(2 * (size_t)(maxl + 2));
-    std::vector<int> planes((size_t)std::min<int64_t>(plane_cap, (int64_t)1 << 31));
-    g.node_cap = N; g.in_pool = EP; g.out_pool = EP;
-    g.base = base.data(); g.aln_n = aln_n.data(); g.aln_id = aln_id.data(); g.in_off = in_off.data(); g.in_n = in_n.data(); g.in_cap = in_cap.data();
-    g.out_off = out_off.data(); g.out_n = out_n.data(); g.out_cap = out_cap.data(); g.in_id = in_id.data(); g.in_w = in_w.data();
-    g.out_id = out_id.data(); g.out_w = out_w.data(); g.out_rid = rid.data(); g.index_to_node = i2n.data(); g.node_to_index = n2i.data();
-    g.remain = remain.data(); g.msa_rank = rank.data(); g.tmp0 = t0.data(); g.tmp1 = t1.data();
-    rt.rec = rrec.data(); rt.pre_row = pre_row.data();
-    d.planes = planes.data(); d.plane_cap = (int64_t)planes.size(); d.row_off = row_off.data(); d.info = rinfo.data();
-    d.cigar = cigar.data(); d.cigar_cap = (int)cigar.size(); d.n_cigar = 0;
-    d.fc = fcache.data(); d.fc_cap = maxl + 2; d.fc_row = -1; d.fc_hi = -1;
+    slot_views(Y, slot.data()->b, planes.data(), g, rt, d);
     graph_reset(g, n_seq);
     std::vector<int64_t> w;
     w.push_back(n_seq); w.push_back(0); w.push_back(0);
@@ -488,7 +479,27 @@ extern "C" int hosttest_flowers(const HtParams *hp, int n_lanes, int n_threads, 
 }
 
 // ---- the device-memory plan of a stage (slot_plan.h), for a given device size ----
-#include "../../cactus_b200/csrc/slot_plan.h"
+// the slot layout for one job: slot_bytes, the 7 capacities (node_cap, in_pool, out_pool, W, cigar_cap, fc_cap, plane_cap),
+// then the 26 offsets in SlotLayout's order
+extern "C" void hosttest_slot_layout(int64_t K, int64_t sum, int64_t ml, int64_t plane_ints, int64_t out[34]) {
+    SlotNeeds need;
+    need.add_job(K, sum, ml, plane_ints);
+    const SlotLayout Y = plan_slot(need);
+    const int64_t v[34] = {Y.slot_bytes, Y.node_cap, Y.in_pool, Y.out_pool, Y.W, Y.cigar_cap, Y.fc_cap, Y.plane_cap,
+                           Y.o_base, Y.o_aln_n, Y.o_aln_id, Y.o_in_off, Y.o_in_n, Y.o_in_cap, Y.o_out_off, Y.o_out_n, Y.o_out_cap,
+                           Y.o_in_id, Y.o_in_w, Y.o_out_id, Y.o_out_w, Y.o_out_rid,
+                           Y.o_index_to_node, Y.o_node_to_index, Y.o_remain, Y.o_msa_rank, Y.o_tmp0, Y.o_tmp1,
+                           Y.o_row_rec, Y.o_pre_row, Y.o_row_off, Y.o_row_info, Y.o_cigar, Y.o_fc};
+    memcpy(out, v, sizeof(v));
+}
+// the guide-tree scratch for one job: slot_bytes, key_cap, base_cap, seq_cap, then the 5 offsets in GtLayout's order
+extern "C" void hosttest_gt_layout(int progressive, int64_t K, int64_t sum, int w, double grow, int worst_case, int64_t out[9]) {
+    GtNeeds need;
+    need.add_job(progressive, K, sum, w, grow, worst_case != 0);
+    const GtLayout Y = plan_gt_scratch(need);
+    const int64_t v[9] = {Y.slot_bytes, Y.key_cap, Y.base_cap, Y.seq_cap, Y.o_keys, Y.o_gx, Y.o_hit, Y.o_jac, Y.o_score};
+    memcpy(out, v, sizeof(v));
+}
 extern "C" int64_t hosttest_plane_ints_for_job(int wb, double wf, int64_t K, int64_t sum, int64_t ml, double grow, int worst_case) {
     return barb200::plane_ints_for_job(wb, wf, K, sum, ml, grow, worst_case != 0);
 }

@@ -56,13 +56,7 @@ int run_jobs_on_lane(barb200_ctx *ctx, int, const std::vector<HostJob> &jobs, st
 }
 }  // namespace barb200
 
-extern "C" void barb200_params_default(barb200_params *p) {
-    static const int mat[25] = {91, -114, -61, -123, -100, -114, 100, -125, -61, -100, -61, -125, 100, -114, -100, -123, -61, -114, 91, -100, -100, -100, -100, -100, 100};
-    memset(p, 0, sizeof(*p));
-    memcpy(p->mat, mat, sizeof(mat));
-    p->gap_open1 = 400; p->gap_ext1 = 30; p->gap_open2 = 1200; p->gap_ext2 = 1; p->wb = 1000; p->wf = 0.1f; p->k = 15; p->w = 5; p->min_w = 500;
-    p->progressive_poa = 1; p->disable_seeding = 1;
-}
+extern "C" void barb200_params_default(barb200_params *p) { barb200::params_default(p); }
 extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *, int) { barb200_ctx *c = new barb200_ctx(); c->p = *p; return c; }
 extern "C" void barb200_destroy(barb200_ctx *ctx) { if (ctx) { barb200::dispatcher_destroy(ctx); delete ctx; } }
 extern "C" const char *barb200_last_error(barb200_ctx *ctx) { static thread_local std::string out; out = ctx ? barb200::get_error(ctx) : "null context"; return out.c_str(); }
