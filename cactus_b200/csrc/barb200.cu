@@ -1,6 +1,6 @@
 // barb200.cu -- device orchestration + C ABI of libbarb200.so (see include/barb200.h).
 //
-// A *stage* is one device batch of POA jobs (one job = one abpoa_msa call of the reference):
+// A *stage* is one device batch of POA jobs (one job = one abpoa_msa call of the reference), planned by stage_plan.h:
 //   * jobs are BUCKETED by the CTA-size class their longest sequence needs (32 .. 1024 threads, 16 columns per thread) and,
 //     inside a class, ordered by estimated cost, largest first. Every class gets its own slot layout sized from ITS largest
 //     job, its own persistent launch on its own stream (largest class first; the launches run concurrently, the block
@@ -24,13 +24,12 @@
 #include <functional>
 #include <memory>
 #include <mutex>
-#include <numeric>
 #include <thread>
 #include <string>
 #include <vector>
 #include "host_api.h"
 #include "poa_kernel.cuh"
-#include "slot_plan.h"
+#include "stage_plan.h"
 
 namespace barb200 {
 extern "C" __global__ void poa_msa_kernel_t32(const BatchArgs A);
@@ -41,13 +40,15 @@ extern "C" __global__ void poa_msa_kernel_t640(const BatchArgs A);
 extern "C" __global__ void poa_msa_kernel_t1024(const BatchArgs A);
 }
 typedef void (*poa_kernel_fn)(const barb200::BatchArgs);
-// CTA-size classes: a CTA of T threads sweeps rows of up to 16*T columns (query length + 1)
-// scratch = dynamic shared memory per CTA (poa_kernel.cuh: poa_scratch_bytes)
-static const struct { int T; poa_kernel_fn fn; int scratch; } kKernels[] = {
+// the kernel of every CTA-size class (stage_plan.h: kClassThreads), scratch = its dynamic shared memory per CTA
+// (poa_kernel.cuh: poa_scratch_bytes)
+static constexpr struct { int T; poa_kernel_fn fn; int scratch; } kKernels[] = {
     {32, barb200::poa_msa_kernel_t32, barb200::poa_scratch_bytes(32)}, {64, barb200::poa_msa_kernel_t64, barb200::poa_scratch_bytes(64)},
     {128, barb200::poa_msa_kernel_t128, barb200::poa_scratch_bytes(128)}, {256, barb200::poa_msa_kernel_t256, barb200::poa_scratch_bytes(256)},
     {640, barb200::poa_msa_kernel_t640, barb200::poa_scratch_bytes(640)}, {1024, barb200::poa_msa_kernel_t1024, barb200::poa_scratch_bytes(1024)}};
-static const int kNumKernels = 6;
+static const int kNumKernels = barb200::kNumClasses;
+static constexpr bool kernels_follow_classes(int i = 0) { return i == kNumKernels || (kKernels[i].T == barb200::kClassThreads[i] && kernels_follow_classes(i + 1)); }
+static_assert(sizeof(kKernels) / sizeof(kKernels[0]) == kNumKernels && kernels_follow_classes(), "kKernels must follow stage_plan.h's classes");
 static const int kMaxDevices = 8;
 using namespace barb200;
 
@@ -210,21 +211,8 @@ static void fail(char *errbuf, int n, const std::string &m) { if (errbuf && n > 
 
 extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *errbuf, int errbuf_len) {
     if (!p) { fail(errbuf, errbuf_len, "null params"); return nullptr; }
-    if (p->gap_open1 <= 0 || p->gap_open2 <= 0 || p->gap_ext1 < 0 || p->gap_ext2 < 0 || (p->gap_ext1 == 0 && p->gap_ext2 == 0)) {
-        fail(errbuf, errbuf_len, "only the convex gap model (both gap opens > 0) is supported; that is what Cactus configures"); return nullptr; }
-    if (p->wb < 0) { fail(errbuf, errbuf_len, "partialOrderAlignmentBandConstant must be >= 0 (adaptive band)"); return nullptr; }
-    if ((int64_t)p->gap_open1 + p->gap_ext1 >= 65535 || (int64_t)p->gap_open2 + p->gap_ext2 >= 65535) {
-        fail(errbuf, errbuf_len, "gap open + extension must be below 65535 (the traceback planes keep E as a 16-bit distance below H)"); return nullptr; }
-    // The sweep's scores are int32, as the reference's are. With every |mat| <= 65535, e <= 65533 < 65534 (from the check above)
-    // and L <= 16383, the largest value it forms, A = H' + (j + 1) e of the F scan, is below 16383 * 65535 + 16384 * 65534 =
-    // 2147368961 < INT32_MAX, and inf_min - min_mis stays above INT32_MIN. Larger scores overflow the reference too (its best
-    // scores then wrap), so there is no answer to reproduce.
-    for (int i = 0; i < 25; ++i)
-        if (p->mat[i] > 65535 || p->mat[i] < -65535) {
-            fail(errbuf, errbuf_len, "partialOrderAlignmentSubMatrix entries must lie in [-65535, 65535] (larger scores overflow the int32 DP "
-                                     "scores, in the reference too)"); return nullptr; }
-    if (!p->disable_seeding) { fail(errbuf, errbuf_len, "minimizer seeding (partialOrderAlignmentDisableSeeding=0) is not supported"); return nullptr; }
-    if (p->k <= 0 || p->k > 20 || p->w <= 0 || p->w >= 256) { fail(errbuf, errbuf_len, "minimizer k must be in 1..20 and w in 1..255 (guide-tree keys are hash << 24 | span << 16 | read)"); return nullptr; }
+    const std::string bad = check_params(*p);
+    if (!bad.empty()) { fail(errbuf, errbuf_len, bad); return nullptr; }
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0) { fail(errbuf, errbuf_len, std::string("no CUDA device: ") + cudaGetErrorString(e)); return nullptr; }
@@ -326,106 +314,27 @@ extern "C" int barb200_device_info(barb200_ctx *ctx, int *sm_count, int64_t *mem
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// stage
+// stage: its plan is stage_plan.h's; here it is measured, allocated, uploaded, launched and fetched
 // ---------------------------------------------------------------------------------------------------------
-// one CTA-size class of a stage: jobs [job_base, job_base + n_jobs) in the stage's internal order
-struct Bucket {
-    int cls = 0, T = 0; size_t dyn_smem = 0;
-    int64_t job_base = 0, n_jobs = 0;
-    SlotLayout lay; int slots = 0;
-    size_t slot_off = 0; int64_t plane_off = 0; size_t clk_off = 0;   // offsets into the lane's arena (bytes / ints / entries)
-};
-
-static int class_of_len(barb200_ctx *ctx, int64_t max_len) {
-    for (int i = 0; i < kNumKernels; ++i) if ((int64_t)kKernels[i].T * CPT >= max_len + 1 && kKernels[i].T >= ctx->p.threads_per_block) return i;
-    return -1;
+// a rejected job table: the context's message, BARB200_EINVAL
+static int table_rc(barb200_ctx *ctx, const std::string &err) {
+    if (err.empty()) return BARB200_OK;
+    set_error(ctx, err); return BARB200_EINVAL;
 }
-// banded cells the job will sweep, roughly: (K-1) alignments x ~mean length rows x band width (SURVEY.md 8e's cost)
-static double job_cost(const barb200_ctx *ctx, int K, int64_t sum, int64_t ml) {
-    const double w = 2.0 * (ctx->P.wb + ctx->P.wf * (double)ml) + 1.0;
-    return (double)(K - 1) * (double)(sum / std::max(1, K) + 1) * std::min<double>((double)ml + 1.0, w) + 2000.0 * K;
-}
-
-// The jobs of one call in the caller's order, scanned and checked once. Stages (and their capacity retries) are lists of indices
-// into it; it keeps its own copy of the lengths because a stage outlives the arguments of barb200_stage_create.
-struct TableJob {
-    int n_seq = 0, max_len = 0, cls = 0, progressive = 0;
-    int64_t len_off = 0, seq_off = 0, sum_len = 0;     // first length in `lens`, first base in the sequence buffer
-    double cost = 0;
-};
-struct JobTable {
-    std::vector<TableJob> jobs;
-    std::vector<int> lens;
-    int64_t n_bases = 0;                                // the sequence buffer: every job's bases back to back
-};
-
-// view(j, len_off, seq_off) -> caller job j, whose lengths and bases the table places at those offsets
-template <class View>
-static int build_table(barb200_ctx *ctx, int64_t n_jobs, View view, JobTable &t) {
-    if (n_jobs > 0x7ffffff0) { set_error(ctx, "too many jobs in one stage"); return BARB200_EINVAL; }
-    t.jobs.resize(n_jobs);
-    int64_t lo = 0, bo = 0;
-    for (int64_t j = 0; j < n_jobs; ++j) {
-        const HostJob v = view(j, lo, bo);
-        if (v.n_seq <= 0) { set_error(ctx, "job without sequences"); return BARB200_EINVAL; }
-        TableJob &J = t.jobs[j];
-        J.n_seq = v.n_seq; J.progressive = v.progressive; J.len_off = lo; J.seq_off = bo;
-        for (int i = 0; i < v.n_seq; ++i) {
-            const int l = v.lens[i];
-            if (l <= 0) { set_error(ctx, "empty sequence in a POA job (the shim substitutes 'N', poaBarAligner.c:551-562)"); return BARB200_EINVAL; }
-            J.sum_len += l; J.max_len = std::max(J.max_len, l);
-        }
-        J.cls = class_of_len(ctx, J.max_len); J.cost = job_cost(ctx, J.n_seq, J.sum_len, J.max_len);
-        if (J.cls < 0) { set_error(ctx, "a sequence is longer than the device engine's row limit (16383 bases per window)"); return BARB200_EINVAL; }
-        if (J.progressive && J.n_seq > 65535) { set_error(ctx, "progressive mode with more than 65535 sequences in one window is not supported"); return BARB200_EINVAL; }
-        t.lens.insert(t.lens.end(), v.lens, v.lens + v.n_seq);
-        lo += v.n_seq; bo += J.sum_len;
-    }
-    t.n_bases = bo;
-    int bad = 0;
-    const int nthreads = host_threads(ctx);
-#pragma omp parallel for schedule(dynamic, 16) num_threads(nthreads) reduction(| : bad)
-    for (int64_t j = 0; j < n_jobs; ++j) {
-        const uint8_t *s = view(j, t.jobs[j].len_off, t.jobs[j].seq_off).seqs;
-        uint8_t m = 0;
-        for (int64_t b = 0; b < t.jobs[j].sum_len; ++b) m |= s[b] > 4;
-        bad |= m;
-    }
-    if (bad) { set_error(ctx, "sequence code > 4"); return BARB200_EINVAL; }
-    return BARB200_OK;
-}
-
-// the jobs as barb200_stage_create and barb200_poa_msa_batch take them: lengths and bases back to back
-static int table_of_arrays(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs, const int *progressive,
-                           JobTable &t) {
-    if (n_jobs < 0 || (n_jobs > 0 && (!n_seq || !seq_lens || !seqs))) { set_error(ctx, "bad arguments"); return BARB200_EINVAL; }
-    return build_table(ctx, n_jobs, [&](int64_t j, int64_t lo, int64_t bo) {
-        return HostJob{n_seq[j], seq_lens + lo, seqs + bo, progressive ? progressive[j] : ctx->hp.progressive_poa};
-    }, t);
-}
-
-static std::vector<int64_t> all_jobs(int64_t n) { std::vector<int64_t> v(n); std::iota(v.begin(), v.end(), (int64_t)0); return v; }
 
 struct barb200_stage {
     barb200_ctx *ctx = nullptr;
     int lane = 0;
     std::shared_ptr<const JobTable> tab;
-    int64_t n_jobs = 0, n_seqs = 0;
-    // everything below is in the stage's INTERNAL job order: class-major (largest class first), cost-descending inside a
-    // class; perm[internal] = the caller's job index in `tab`
-    std::vector<int64_t> perm;
-    std::vector<int> lens;
-    std::vector<int64_t> soff;
-    std::vector<JobDesc> desc;
-    std::vector<Bucket> buckets;
-    int64_t msa_bytes = 0;
-    double grow = 1.0; bool worst_case = false;
+    int64_t n_jobs = 0;
+    StagePlan plan;
+    std::vector<size_t> dyn_smem;                                    // per bucket: dynamic shared memory per CTA
     // device: one block from the device's cache holds all per-stage arrays; a retry's d_seqs are its first stage's
-    void *d_block = nullptr; size_t d_block_bytes = 0;
+    void *d_block = nullptr;
     uint8_t *d_seqs = nullptr, *d_msa = nullptr; int *d_lens = nullptr; int64_t *d_soff = nullptr;
     JobDesc *d_desc = nullptr; int *d_msa_len = nullptr, *d_status = nullptr, *d_next = nullptr; long long *d_cells = nullptr;
     int *d_order = nullptr, *d_gt_status = nullptr; uint8_t *d_gt_scratch = nullptr;
-    GuideTreeArgs gt; int gt_ctas = 0; cudaEvent_t e_gt = nullptr;   // K0: the guide trees of the stage (guide_tree.cu)
+    GuideTreeArgs gt; cudaEvent_t e_gt = nullptr;                    // K0: the guide trees of the stage (guide_tree.cu)
     std::vector<int> status;                                         // of the last run
     std::vector<std::unique_ptr<barb200_stage>> retries;             // the last run's capacity retries: x4, then worst case
     int64_t launches = 0; bool ran = false;
@@ -436,70 +345,39 @@ struct barb200_stage {
         retries.clear();
         if (e0) { cudaEventDestroy(e0); cudaEventDestroy(e1); }
         if (e_gt) cudaEventDestroy(e_gt);
-        dev_free(dev_of_lane(ctx, lane), d_block, d_block_bytes);
+        dev_free(dev_of_lane(ctx, lane), d_block, (size_t)plan.block_bytes);
     }
 };
 
 extern "C" void barb200_stage_destroy(barb200_stage *st) { delete st; }
 
-// Slot sizes, shared memory and resident CTAs of every bucket; carve the lane's arena.
+// Shared memory and resident CTAs of every bucket, and the memory the lane may plan with; fit_stage sizes the slots from them.
 static int plan_stage(barb200_stage *st) {
     barb200_ctx *ctx = st->ctx;
     Device &D = dev_of_lane(ctx, st->lane);
     Lane &LN = lane_of(ctx, st->lane);
-    for (Bucket &B : st->buckets) {
-        SlotNeeds need;
-        for (int64_t j = B.job_base; j < B.job_base + B.n_jobs; ++j) {
-            const TableJob &J = st->tab->jobs[st->perm[j]];
-            need.add_job(J.n_seq, J.sum_len, J.max_len, plane_ints_for_job(ctx->P.wb, ctx->P.wf, J.n_seq, J.sum_len, J.max_len, st->grow, st->worst_case));
-        }
-        B.lay = plan_slot(need);
-        B.T = kKernels[B.cls].T; B.dyn_smem = kKernels[B.cls].scratch;
-        if (getenv("BARB200_SCRATCH_KB")) B.dyn_smem = (size_t)atoi(getenv("BARB200_SCRATCH_KB")) * 1024;   // tuning aid
+    std::vector<int> per_sm(st->plan.buckets.size(), 0);
+    st->dyn_smem.assign(st->plan.buckets.size(), 0);
+    for (size_t b = 0; b < st->plan.buckets.size(); ++b) {
+        const PlanBucket &B = st->plan.buckets[b];
+        size_t smem = kKernels[B.cls].scratch;
+        if (getenv("BARB200_SCRATCH_KB")) smem = (size_t)atoi(getenv("BARB200_SCRATCH_KB")) * 1024;   // tuning aid
         // never below the sweep's ring, which the kernel uses without a run-time check (the topological sort and the MSA ranking
         // fit whatever is left, falling back to global memory)
-        B.dyn_smem = std::max(B.dyn_smem, (size_t)poa_ring_bytes(B.T));
-        int per_sm = 0;
-        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kKernels[B.cls].fn, B.T, B.dyn_smem));
-        if (per_sm < 1) { set_error(ctx, "kernel does not fit on an SM with the requested configuration"); return BARB200_EINVAL; }
-        if (ctx->p.ctas_per_sm > 0) per_sm = std::min(per_sm, ctx->p.ctas_per_sm);
-        B.slots = (int)std::min<int64_t>(B.n_jobs, (int64_t)per_sm * D.sm_count);
+        smem = std::max(smem, (size_t)poa_ring_bytes(B.T));
+        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[b], kKernels[B.cls].fn, B.T, smem));
+        if (per_sm[b] < 1) { set_error(ctx, "kernel does not fit on an SM with the requested configuration"); return BARB200_EINVAL; }
+        if (ctx->p.ctas_per_sm > 0) per_sm[b] = std::min(per_sm[b], ctx->p.ctas_per_sm);
+        st->dyn_smem[b] = smem;
     }
     // memory: what is free now + what this lane's arena already holds, minus the stage's own block; a lane of a context
     // whose dispatcher runs plans with its share so that the other lane of the device can do the same
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(ctx, cudaMemGetInfo(&free_b, &total_b));
-    const double frac = ctx->p.mem_fraction > 0 ? ctx->p.mem_fraction : 0.85;
-    const double budget = lane_budget_bytes((double)free_b, (double)total_b, (double)(LN.slots_bytes + LN.planes_bytes), (double)st->d_block_bytes,
-                                            frac, ctx->lanes_shared, ctx->lanes_per_device);
-    auto need_of = [&](const Bucket &B) { return (double)B.slots * ((double)B.lay.slot_bytes + (double)B.lay.plane_cap * 4.0); };
-    double need = 0;
-    for (const Bucket &B : st->buckets) need += need_of(B);
-    for (int pass = 0; pass < 8 && need > budget; ++pass) {
-        const double scale = budget / need;
-        need = 0;
-        for (Bucket &B : st->buckets) { B.slots = std::max(1, (int)((double)B.slots * scale)); need += need_of(B); }
-    }
-    if (need > budget && (st->grow > 1.0 || st->worst_case)) {
-        double fixed = 0, planes = 0;
-        for (const Bucket &B : st->buckets) { fixed += (double)B.slots * (double)B.lay.slot_bytes; planes += (double)B.slots * (double)B.lay.plane_cap * 4.0; }
-        const double scale = retry_plane_scale(budget, fixed, planes);
-        need = 0;
-        for (Bucket &B : st->buckets) {
-            B.lay.plane_cap = (int64_t)((double)B.lay.plane_cap * scale) / 8 * 8;
-            need += need_of(B);
-        }
-    }
-    if (need > budget) {
-        char buf[200];
-        snprintf(buf, sizeof(buf), "a single job needs more device memory than is available (%.1f GB planned, %.1f GB usable by this lane)", need / 1e9, budget / 1e9);
-        set_error(ctx, buf); return BARB200_ENOMEM;
-    }
-    size_t so = 0, co = 0; int64_t po = 0;
-    for (Bucket &B : st->buckets) {
-        B.slot_off = so; B.plane_off = po; B.clk_off = co;
-        so += (size_t)B.lay.slot_bytes * B.slots; po += B.lay.plane_cap * B.slots; co += (size_t)B.slots * PH_N;
-    }
+    const double budget = lane_budget_bytes((double)free_b, (double)total_b, (double)(LN.slots_bytes + LN.planes_bytes), (double)st->plan.block_bytes,
+                                            ctx_mem_fraction(ctx), ctx->lanes_shared, ctx->lanes_per_device);
+    const std::string err = fit_stage(st->plan, per_sm, D.sm_count, budget);
+    if (!err.empty()) { set_error(ctx, err); return BARB200_ENOMEM; }
     return BARB200_OK;
 }
 
@@ -545,71 +423,37 @@ static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTabl
     Lane &LN = lane_of(ctx, lane);
     cudaSetDevice(D.ordinal);
     std::unique_ptr<barb200_stage> st(new barb200_stage());
-    const JobTable &T = *tab;
     const int64_t n_jobs = (int64_t)jobs.size();
-    st->ctx = ctx; st->lane = lane; st->tab = std::move(tab); st->n_jobs = n_jobs; st->grow = grow; st->worst_case = worst_case;
+    st->ctx = ctx; st->lane = lane; st->tab = std::move(tab); st->n_jobs = n_jobs;
     const double tb0 = now_ms();
-    // ---- internal order: largest class first, inside a class by estimated cost, largest first (stable) ----
-    st->perm = std::move(jobs);
-    std::stable_sort(st->perm.begin(), st->perm.end(), [&](int64_t a, int64_t b) {
-        if (T.jobs[a].cls != T.jobs[b].cls) return T.jobs[a].cls > T.jobs[b].cls;
-        return T.jobs[a].cost > T.jobs[b].cost;
-    });
-    st->desc.resize(n_jobs);
-    int64_t lo = 0, msa_off = 0;
-    for (int64_t j = 0; j < n_jobs; ++j) {
-        const TableJob &J = T.jobs[st->perm[j]];
-        const int K = J.n_seq;
-        int64_t o = 0;
-        for (int i = 0; i < K; ++i) { st->lens.push_back(T.lens[J.len_off + i]); st->soff.push_back(o); o += T.lens[J.len_off + i]; }
-        int64_t stride = J.sum_len;
-        if (!worst_case) stride = std::min<int64_t>(J.sum_len, (int64_t)(grow * (double)(J.max_len + J.max_len / 2 + 64)));
-        stride = align_up(stride, 16);
-        JobDesc &d = st->desc[j];
-        d.n_seq = K; d.seq_off = J.seq_off; d.len_off = lo; d.msa_off = msa_off; d.msa_stride = (int)stride; d.progressive = J.progressive;
-        msa_off += stride * K;
-        lo += K;
-        if (st->buckets.empty() || st->buckets.back().cls != J.cls) { Bucket B; B.cls = J.cls; B.job_base = j; st->buckets.push_back(B); }
-        st->buckets.back().n_jobs++;
-    }
-    const int64_t ns = st->n_seqs = lo;
-    st->msa_bytes = msa_off;
+    const StagePlan &S = st->plan = plan_stage_order(*st->tab, std::move(jobs), ctx->p, grow, worst_case, D.sm_count, d_seqs == nullptr);
     if (n_jobs == 0) { *out = st.release(); return BARB200_OK; }
-    // K0's scratch: one slot per resident guide-tree CTA, sized from the stage's largest job
-    GuideTreeArgs &GA = st->gt;
-    memset(&GA, 0, sizeof(GA));
-    GtNeeds gt_need;
-    for (int64_t c : st->perm) gt_need.add_job(T.jobs[c].progressive, T.jobs[c].n_seq, T.jobs[c].sum_len, ctx->p.w, grow, worst_case);
-    GA.lay = plan_gt_scratch(gt_need);
-    st->gt_ctas = (int)std::min<int64_t>(std::min<int64_t>(n_jobs, (int64_t)4 * D.sm_count), std::max<int64_t>(1, ((int64_t)2 << 30) / GA.lay.slot_bytes));
-    // device buffers (one cached block) + upload on the lane's copy stream, so that it overlaps a running kernel
-    BumpOffsets sub{256};
-    const int64_t o_seqs = d_seqs ? 0 : sub.take(T.n_bases), o_lens = sub.take(ns * 4), o_soff = sub.take(ns * 8), o_desc = sub.take(n_jobs * sizeof(JobDesc)),
-                  o_msa = sub.take(st->msa_bytes), o_msa_len = sub.take(n_jobs * 4), o_status = sub.take(n_jobs * 4), o_cells = sub.take(n_jobs * 8),
-                  o_next = sub.take(4 * (kNumKernels + 1)), o_order = sub.take(ns * 4), o_gts = sub.take(n_jobs * 4), o_gtscr = sub.take(GA.lay.slot_bytes * st->gt_ctas);
-    st->d_block_bytes = (size_t)sub.end;
     const double tb2 = now_ms();
     int rc = plan_stage(st.get());
     if (rc) return rc;
     const double tb3 = now_ms();
-    cudaError_t e = dev_alloc(D, &st->d_block, st->d_block_bytes);
+    // device buffers (one cached block) + upload on the lane's copy stream, so that it overlaps a running kernel
+    cudaError_t e = dev_alloc(D, &st->d_block, (size_t)S.block_bytes);
     if (e != cudaSuccess) {
         cudaGetLastError(); set_error(ctx, std::string("cudaMalloc(stage) failed: ") + cudaGetErrorString(e));
         st->d_block = nullptr; return BARB200_ENOMEM;
     }
     uint8_t *blk = (uint8_t *)st->d_block;
-    st->d_seqs = d_seqs ? d_seqs : blk + o_seqs; st->d_lens = (int *)(blk + o_lens); st->d_soff = (int64_t *)(blk + o_soff);
-    st->d_desc = (JobDesc *)(blk + o_desc); st->d_msa = blk + o_msa; st->d_msa_len = (int *)(blk + o_msa_len); st->d_status = (int *)(blk + o_status);
-    st->d_cells = (long long *)(blk + o_cells); st->d_next = (int *)(blk + o_next);
-    st->d_order = (int *)(blk + o_order); st->d_gt_status = (int *)(blk + o_gts); st->d_gt_scratch = blk + o_gtscr;
+    st->d_seqs = d_seqs ? d_seqs : blk + S.o_seqs; st->d_lens = (int *)(blk + S.o_lens); st->d_soff = (int64_t *)(blk + S.o_soff);
+    st->d_desc = (JobDesc *)(blk + S.o_desc); st->d_msa = blk + S.o_msa; st->d_msa_len = (int *)(blk + S.o_msa_len); st->d_status = (int *)(blk + S.o_status);
+    st->d_cells = (long long *)(blk + S.o_cells); st->d_next = (int *)(blk + S.o_next);
+    st->d_order = (int *)(blk + S.o_order); st->d_gt_status = (int *)(blk + S.o_gt_status); st->d_gt_scratch = blk + S.o_gt_scratch;
+    GuideTreeArgs &GA = st->gt;
+    memset(&GA, 0, sizeof(GA));
     GA.jobs = st->d_desc; GA.n_jobs = (int)n_jobs; GA.seqs = st->d_seqs; GA.lens = st->d_lens; GA.soff = st->d_soff; GA.order = st->d_order; GA.gt_status = st->d_gt_status;
-    GA.next_job = st->d_next + kNumKernels; GA.scratch = st->d_gt_scratch; GA.k = ctx->p.k; GA.w = ctx->p.w;
+    GA.next_job = st->d_next + kNumKernels; GA.scratch = st->d_gt_scratch; GA.lay = S.gt; GA.k = ctx->p.k; GA.w = ctx->p.w;
     cudaStream_t s = LN.copy;
+    const int64_t ns = S.n_seqs;
     const double tb4 = now_ms();
-    if ((!d_seqs && (e = cudaMemcpyAsync(st->d_seqs, seqs, T.n_bases, cudaMemcpyHostToDevice, s)) != cudaSuccess) ||
-        (e = cudaMemcpyAsync(st->d_lens, st->lens.data(), ns * 4, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
-        (e = cudaMemcpyAsync(st->d_soff, st->soff.data(), ns * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
-        (e = cudaMemcpyAsync(st->d_desc, st->desc.data(), n_jobs * sizeof(JobDesc), cudaMemcpyHostToDevice, s)) != cudaSuccess ||
+    if ((!d_seqs && (e = cudaMemcpyAsync(st->d_seqs, seqs, st->tab->n_bases, cudaMemcpyHostToDevice, s)) != cudaSuccess) ||
+        (e = cudaMemcpyAsync(st->d_lens, S.lens.data(), ns * 4, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
+        (e = cudaMemcpyAsync(st->d_soff, S.soff.data(), ns * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
+        (e = cudaMemcpyAsync(st->d_desc, S.desc.data(), n_jobs * sizeof(JobDesc), cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaStreamSynchronize(s)) != cudaSuccess) {
         set_error(ctx, std::string("H2D failed: ") + cudaGetErrorString(e)); return BARB200_ECUDA;
     }
@@ -623,7 +467,7 @@ extern "C" int barb200_stage_create(barb200_ctx *ctx, int64_t n_jobs, const int 
                                     const uint8_t *seqs, const int *progressive, barb200_stage **out) {
     if (!ctx || !out) return BARB200_EINVAL;
     auto tab = std::make_shared<JobTable>();
-    const int rc = table_of_arrays(ctx, n_jobs, n_seq, seq_lens, seqs, progressive, *tab);
+    const int rc = table_rc(ctx, table_of_arrays(ctx->p, host_threads(ctx), n_jobs, n_seq, seq_lens, seqs, progressive, *tab));
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(lane_of(ctx, 0).busy);
     return stage_build(ctx, 0, tab, all_jobs(n_jobs), 1.0, false, seqs, nullptr, out);
@@ -638,26 +482,25 @@ static int stage_launch(barb200_stage *st) {
     st->launches = 0; st->ran = false; st->launched = false;
     if (st->n_jobs == 0) return BARB200_OK;
     st->retries.clear();
-    size_t slots_bytes = 0, plane_ints = 0, clk_n = 0;
-    for (const Bucket &B : st->buckets) { slots_bytes += (size_t)B.lay.slot_bytes * B.slots; plane_ints += (size_t)B.lay.plane_cap * B.slots; clk_n += (size_t)B.slots * PH_N; }
-    if (!ctx->p.collect_phase_clocks) clk_n = 0;
-    int rc = ensure_arena(ctx, dev_of_lane(ctx, st->lane), LN, slots_bytes, plane_ints * 4, clk_n);
+    const StagePlan &S = st->plan;
+    const size_t clk_n = ctx->p.collect_phase_clocks ? S.clk_entries : 0;
+    int rc = ensure_arena(ctx, dev_of_lane(ctx, st->lane), LN, S.slots_bytes, S.plane_ints * 4, clk_n);
     if (rc) return rc;
     cudaStream_t s = LN.main;
     CUDA_TRY(ctx, cudaMemsetAsync(st->d_next, 0, 4 * (kNumKernels + 1), s));
-    CUDA_TRY(ctx, cudaMemsetAsync(st->d_msa, 0, st->msa_bytes, s));     // the rows' padding travels back with the MSAs (one D2H copy): defined bytes
+    CUDA_TRY(ctx, cudaMemsetAsync(st->d_msa, 0, S.msa_bytes, s));     // the rows' padding travels back with the MSAs (one D2H copy): defined bytes
     if (clk_n) CUDA_TRY(ctx, cudaMemsetAsync(LN.d_clk, 0, clk_n * sizeof(unsigned long long), s));
     if (!st->e0) { CUDA_TRY(ctx, cudaEventCreate(&st->e0)); CUDA_TRY(ctx, cudaEventCreate(&st->e1)); }
     if (!st->e_gt) CUDA_TRY(ctx, cudaEventCreate(&st->e_gt));
     CUDA_TRY(ctx, cudaEventRecord(st->e0, s));
     // K0: the guide trees of every job (guide_tree.cu); the POA launches below wait for it through the stream / e_gt
-    launch_guide_tree(st->gt, st->gt_ctas, (void *)s);
+    launch_guide_tree(st->gt, S.gt_ctas, (void *)s);
     { cudaError_t le = cudaGetLastError(); if (le != cudaSuccess) { set_error(ctx, std::string("guide tree launch: ") + cudaGetErrorString(le)); return BARB200_ECUDA; } }
     CUDA_TRY(ctx, cudaEventRecord(st->e_gt, s));
     st->launches++;
-    const bool single = st->buckets.size() == 1;
-    for (size_t b = 0; b < st->buckets.size(); ++b) {          // largest class first
-        const Bucket &B = st->buckets[b];
+    const bool single = S.buckets.size() == 1;
+    for (size_t b = 0; b < S.buckets.size(); ++b) {          // largest class first
+        const PlanBucket &B = S.buckets[b];
         BatchArgs A;
         A.jobs = st->d_desc; A.job_base = (int)B.job_base; A.n_jobs = (int)B.n_jobs; A.seqs = st->d_seqs; A.lens = st->d_lens; A.soff = st->d_soff;
         A.order = st->d_order; A.gt_status = st->d_gt_status;
@@ -666,10 +509,10 @@ static int stage_launch(barb200_stage *st) {
         A.phase_clk = clk_n ? LN.d_clk + B.clk_off : nullptr;
         A.serial_phases = getenv("BARB200_DEBUG_SERIAL") ? 1 : 0;
         A.bfs_order = getenv("BARB200_DEBUG_BFS") ? 1 : 0;
-        A.scratch_bytes = (int)B.dyn_smem; A.lay = B.lay; A.P = ctx->P;
+        A.scratch_bytes = (int)st->dyn_smem[b]; A.lay = B.lay; A.P = ctx->P;
         cudaStream_t cs = single ? s : LN.cls[B.cls];
         if (!single) CUDA_TRY(ctx, cudaStreamWaitEvent(cs, st->e_gt, 0));
-        kKernels[B.cls].fn<<<B.slots, B.T, B.dyn_smem, cs>>>(A);
+        kKernels[B.cls].fn<<<B.slots, B.T, st->dyn_smem[b], cs>>>(A);
         cudaError_t le = cudaGetLastError();
         if (le != cudaSuccess) { set_error(ctx, std::string("kernel launch: ") + cudaGetErrorString(le)); return BARB200_ECUDA; }
         if (!single) { CUDA_TRY(ctx, cudaEventRecord(LN.cls_done[B.cls], cs)); CUDA_TRY(ctx, cudaStreamWaitEvent(s, LN.cls_done[B.cls], 0)); }
@@ -707,32 +550,18 @@ static int stage_finish(barb200_stage *st, float *kernel_ms) {
         CUDA_TRY(ctx, cudaStreamSynchronize(s));
         st->clk[6] += (uint64_t)(gt_ms * 1e6f);          // K0 is a kernel of its own: its device time, in nanoseconds
         if (ctx->p.collect_phase_clocks) {
-            size_t clk_n = 0;
-            for (const Bucket &B : r->buckets) clk_n += (size_t)B.slots * PH_N;
+            const size_t clk_n = r->plan.clk_entries;
             std::vector<unsigned long long> h(clk_n);
             CUDA_TRY(ctx, cudaMemcpy(h.data(), LN.d_clk, clk_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
             for (size_t b = 0; b < clk_n / PH_N; ++b) for (int k = 0; k < 6; ++k) st->clk[k] += h[b * PH_N + k];
         }
         // capacity misses -> retry launch for just those jobs with larger slots (x4 first, then worst case)
-        std::vector<int64_t> redo;
-        for (int64_t j = 0; j < r->n_jobs; ++j) {
-            const int sc = r->status[j];
-            if (sc == JOB_OK) continue;
-            if (!r->worst_case && (sc == JOB_ERR_PLANE_CAP || sc == JOB_ERR_MSA_CAP || sc == JOB_ERR_GT_CAP)) redo.push_back(r->perm[j]);
-            else {
-                char buf[200];
-                if (sc == JOB_ERR_PLANE_CAP)
-                    snprintf(buf, sizeof(buf), "job %lld needs more DP-plane memory than this lane can plan (%.1f GB of planes per slot)", (long long)r->perm[j],
-                             r->buckets.empty() ? 0.0 : (double)r->buckets[0].lay.plane_cap * 4.0 / 1e9);
-                else
-                    snprintf(buf, sizeof(buf), "job %lld failed on the device with status %d", (long long)r->perm[j], sc);
-                set_error(ctx, buf); return BARB200_EJOB;
-            }
-        }
-        if (redo.empty()) break;
+        RetryRound next;
+        const std::string err = retry_round(r->plan, r->status, next);
+        if (!err.empty()) { set_error(ctx, err); return BARB200_EJOB; }
+        if (next.jobs.empty()) break;
         barb200_stage *rs = nullptr;
-        const bool go_worst = r->grow >= 4.0;
-        int rc = stage_build(ctx, st->lane, st->tab, std::move(redo), go_worst ? 1.0 : r->grow * 4.0, go_worst, nullptr, st->d_seqs, &rs);
+        int rc = stage_build(ctx, st->lane, st->tab, std::move(next.jobs), next.grow, next.worst_case, nullptr, st->d_seqs, &rs);
         if (rc) return rc;
         st->retries.emplace_back(rs);
         if ((rc = stage_launch(rs))) return rc;
@@ -763,7 +592,7 @@ extern "C" int barb200_stage_phase_clocks(barb200_stage *st, uint64_t out[7]) {
 extern "C" int barb200_stage_buckets(barb200_stage *st, int64_t *out, int max_buckets) {
     if (!st) return 0;
     int n = 0;
-    for (const Bucket &B : st->buckets) {
+    for (const PlanBucket &B : st->plan.buckets) {
         if (n >= max_buckets) break;
         if (out) { out[4 * n] = B.T; out[4 * n + 1] = B.n_jobs; out[4 * n + 2] = B.slots; out[4 * n + 3] = B.lay.plane_cap; }
         ++n;
@@ -786,28 +615,29 @@ static int stage_fetch_locked(barb200_stage *st, const MsaDest &dest, int *msa_l
     for (auto &rs : st->retries) rounds.push_back(rs.get());
     for (barb200_stage *r : rounds) {
         std::vector<int> r_len(r->n_jobs); std::vector<long long> r_cells(r->n_jobs);
-        PinnedBlock down(D, (size_t)r->msa_bytes);
+        PinnedBlock down(D, (size_t)r->plan.msa_bytes);
         if (!down.p) { set_error(ctx, "cudaMallocHost failed"); return BARB200_ENOMEM; }
         uint8_t *h_msa = (uint8_t *)down.p;
         cudaStream_t s = LN.main;
         CUDA_TRY(ctx, cudaMemcpyAsync(r_len.data(), r->d_msa_len, r->n_jobs * 4, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(ctx, cudaMemcpyAsync(r_cells.data(), r->d_cells, r->n_jobs * 8, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(ctx, cudaMemcpyAsync(h_msa, r->d_msa, r->msa_bytes, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaMemcpyAsync(h_msa, r->d_msa, r->plan.msa_bytes, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(ctx, cudaStreamSynchronize(s));
         int oom = 0;
         const int nthreads = host_threads(ctx);
 #pragma omp parallel for schedule(static) num_threads(nthreads) reduction(| : oom)
         for (int64_t j = 0; j < r->n_jobs; ++j) {
             if (r->status[j] != JOB_OK) continue;           // re-run by a later round
-            const int64_t c = r->perm[j];
-            const int K = r->desc[j].n_seq, ml = r_len[j];
+            const JobDesc &d = r->plan.desc[j];
+            const int64_t c = r->plan.perm[j];
+            const int K = d.n_seq, ml = r_len[j];
             if (msa_len) msa_len[c] = ml;
             if (cells) cells[c] = r_cells[j];
             if (dest) {
                 uint8_t *o = dest(c, K, ml);
                 if (!o) { oom = 1; continue; }
-                const uint8_t *src = h_msa + r->desc[j].msa_off;
-                for (int i = 0; i < K; ++i) memcpy(o + (size_t)i * ml, src + (size_t)i * r->desc[j].msa_stride, ml);
+                const uint8_t *src = h_msa + d.msa_off;
+                for (int i = 0; i < K; ++i) memcpy(o + (size_t)i * ml, src + (size_t)i * d.msa_stride, ml);
             }
         }
         if (oom) { set_error(ctx, "host allocation failed"); return BARB200_ENOMEM; }
@@ -853,30 +683,16 @@ static int batch_on_lane(barb200_ctx *ctx, int lane, const std::shared_ptr<const
     return rc;
 }
 
-// job-count / byte limits of ONE device batch (larger requests are cut into chunks)
-static const int64_t kMaxJobsPerBatch = 1 << 15;
-static const int64_t kMaxBasesPerBatch = (int64_t)768 << 20;
-
 extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens,
                                      const uint8_t *seqs, const int *progressive, uint8_t **msa_out, int *msa_len,
                                      int64_t *cells) {
     if (!ctx) return BARB200_EINVAL;
     if (msa_out) for (int64_t j = 0; j < n_jobs; ++j) msa_out[j] = nullptr;
     auto tab = std::make_shared<JobTable>();
-    const int trc = table_of_arrays(ctx, n_jobs, n_seq, seq_lens, seqs, progressive, *tab);
+    const int trc = table_rc(ctx, table_of_arrays(ctx->p, host_threads(ctx), n_jobs, n_seq, seq_lens, seqs, progressive, *tab));
     if (trc || n_jobs == 0) return trc;
-    const std::vector<TableJob> &J = tab->jobs;
     const int ndev = (int)ctx->devs.size();
-    // ---- deal: one device -> everything; several -> cost-sorted, each job to the device with the least work so far (LPT, SURVEY.md 8e) ----
-    std::vector<std::vector<int64_t>> share(ndev);
-    if (ndev == 1) share[0] = all_jobs(n_jobs);
-    else {
-        std::vector<int64_t> idx = all_jobs(n_jobs);
-        std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return J[a].cost > J[b].cost; });
-        std::vector<double> load(ndev, 0.0);
-        for (int64_t j : idx) { const int d = (int)(std::min_element(load.begin(), load.end()) - load.begin()); share[d].push_back(j); load[d] += J[j].cost; }
-        for (auto &s : share) std::sort(s.begin(), s.end());
-    }
+    const std::vector<std::vector<int64_t>> share = deal_jobs(*tab, ndev);
     std::vector<int> rcs(ndev, BARB200_OK);
     std::vector<std::string> errs(ndev);
     int active_devs = 0;
@@ -887,12 +703,7 @@ extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int
         const int lane = d * ctx->lanes_per_device;
         std::lock_guard<std::mutex> lk(lane_of(ctx, lane).busy);
         size_t at = 0;
-        while (at < mine.size() && rcs[d] == BARB200_OK) {
-            // one chunk: a bounded number of jobs and bases
-            size_t end = at; int64_t bases = 0;
-            while (end < mine.size() && (int64_t)(end - at) < kMaxJobsPerBatch && (end == at || bases + J[mine[end]].sum_len <= kMaxBasesPerBatch)) {
-                bases += J[mine[end]].sum_len; ++end;
-            }
+        for (size_t end : chunk_ends(*tab, mine)) {
             const int rc = batch_on_lane(ctx, lane, tab, std::vector<int64_t>(mine.begin() + at, mine.begin() + end), seqs, malloc_dest(msa_out), msa_len, cells);
             if (rc) { rcs[d] = rc; errs[d] = get_error(ctx); break; }
             at = end;
@@ -928,7 +739,7 @@ int run_jobs_on_lane(barb200_ctx *ctx, int lane, const std::vector<HostJob> &job
     results.assign(n, JobResult());
     if (n == 0) return BARB200_OK;
     auto tab = std::make_shared<JobTable>();
-    int rc = build_table(ctx, n, [&](int64_t j, int64_t, int64_t) { return jobs[j]; }, *tab);
+    int rc = table_rc(ctx, build_table(ctx->p, host_threads(ctx), n, [&](int64_t j, int64_t, int64_t) { return jobs[j]; }, *tab));
     if (rc) return rc;
     const std::vector<TableJob> &J = tab->jobs;
     Lane &LN = lane_of(ctx, lane);

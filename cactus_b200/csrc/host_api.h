@@ -19,6 +19,12 @@ inline void params_default(barb200_params *p) {
     p->k = 15; p->w = 5; p->min_w = 500;
     p->progressive_poa = 1; p->disable_seeding = 1;
 }
+// barb200_pecan_params_default: pairwiseAlignmentBandingParameters_construct, pairwiseAligner.c:1369-1391
+inline void pecan_params_default(barb200_pecan_params *p) {
+    memset(p, 0, sizeof(*p));
+    p->threshold = 0.01; p->min_diags_between_traceback = 1000; p->traceback_diagonals = 40; p->diagonal_expansion = 20;
+    p->split_matrix_bigger_than_this = (int64_t)3000 * 3000; p->dynamic_anchor_expansion = 0;
+}
 
 struct HostParams {
     int k, w, min_w, progressive_poa;

@@ -186,11 +186,7 @@ struct barb200_pecan_stage {
     std::vector<Block> blocks;                   // the stage's own device arrays, from the context's block cache
 };
 
-extern "C" void barb200_pecan_params_default(barb200_pecan_params *p) {
-    memset(p, 0, sizeof(*p));            // pairwiseAlignmentBandingParameters_construct, pairwiseAligner.c:1369-1391
-    p->threshold = 0.01; p->min_diags_between_traceback = 1000; p->traceback_diagonals = 40; p->diagonal_expansion = 20;
-    p->split_matrix_bigger_than_this = (int64_t)3000 * 3000; p->dynamic_anchor_expansion = 0;
-}
+extern "C" void barb200_pecan_params_default(barb200_pecan_params *p) { pecan_params_default(p); }
 
 static inline int sym_of(char c) {       // symbol_convertCharToSymbol, pairwiseAligner.c:327-344
     switch (c) { case 'A': case 'a': return 0; case 'C': case 'c': return 1; case 'G': case 'g': return 2; case 'T': case 't': return 3; default: return 4; }

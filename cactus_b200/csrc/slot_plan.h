@@ -1,4 +1,4 @@
-// slot_plan.h -- the arithmetic of a stage's device-memory plan (barb200.cu: plan_stage) and the layout of the memory it plans:
+// slot_plan.h -- the arithmetic of a stage's device-memory plan (stage_plan.h: fit_stage) and the layout of the memory it plans:
 // a POA slot, a guide-tree scratch slot. CUDA-free, so that the CPU suite runs the product's graph and guide-tree code on the
 // same layout (tests/hosttest) and checks the plan for a given device size.
 #pragma once

@@ -391,6 +391,36 @@ extern "C" long long hosttest_batch_merge_stress(int threads, int iters, long lo
 
 
 // ---------------------------------------------------------------------------------------------------------
+// one device batch on the CPU: the product's job table and stage order (stage_plan.h), every job computed by
+// hosttest_poa_msa_trace in the stage's internal order and its result written at the caller's index. The stand-in device
+// (standin_device.cpp) and hosttest_flowers run their batches through it, so they reject what the product rejects.
+// ---------------------------------------------------------------------------------------------------------
+#include "../../cactus_b200/csrc/stage_plan.h"
+
+int hosttest_device_batch(const HtParams &hp, int threads_per_block, const std::vector<HostJob> &jobs, std::vector<JobResult> &res, std::string &err) {
+    res.assign(jobs.size(), JobResult());
+    barb200_params p;
+    params_default(&p);
+    p.wb = hp.wb; p.wf = hp.wf; p.w = hp.w; p.progressive_poa = hp.progressive; p.threads_per_block = threads_per_block;
+    JobTable T;
+    err = build_table(p, 4, (int64_t)jobs.size(), [&](int64_t j, int64_t, int64_t) { return jobs[j]; }, T);
+    if (!err.empty()) return BARB200_EINVAL;
+    const StagePlan S = plan_stage_order(T, all_jobs((int64_t)jobs.size()), p, 1.0, false, 1, true);
+    for (const int64_t c : S.perm) {
+        HtParams q = hp; q.progressive = T.jobs[c].progressive;
+        int64_t nw = 0; int status = 0;
+        int64_t *w = hosttest_poa_msa_trace(&q, jobs[c].n_seq, jobs[c].lens, jobs[c].seqs, &nw, &status);
+        if (status) { free(w); err = "stand-in device: job failed"; return BARB200_EJOB; }
+        const int ml = (int)w[1];
+        const size_t nb = (size_t)jobs[c].n_seq * ml, nwm = (nb + 7) / 8;
+        res[c].msa.assign((const uint8_t *)(w + (nw - (int64_t)nwm)), (const uint8_t *)(w + (nw - (int64_t)nwm)) + nb);
+        res[c].msa_len = ml; res[c].cells = w[2];
+        free(w);
+    }
+    return BARB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // end_queue.h + bar_windows.h: the product's end queue (tickets, lane workers, window rounds, trimming, stitching, cross-end
 // consistency) driven by application threads, with a stand-in device: every job's MSA comes from the host build of the
 // product's graph code above (hosttest_poa_msa_trace). flowers: n_flowers tickets; flat description as in the arguments.
@@ -403,25 +433,10 @@ extern "C" int hosttest_flowers(const HtParams *hp, int n_lanes, int n_threads, 
                                 const int64_t *ov, int64_t window_size, int64_t max_prog_rows, double max_prog_length_diff,
                                 int64_t *col_out, uint8_t **msa_out, int64_t *batches_out, int *ticket_rc) {
     std::atomic<long long> calls(0);
-    barb200::EndQueue::Exec exec = [&](int lane, const std::vector<barb200::HostJob> &jobs, std::vector<barb200::JobResult> &res, std::string &err) -> int {
-        (void)lane;
+    barb200::EndQueue::Exec exec = [&](int, const std::vector<barb200::HostJob> &jobs, std::vector<barb200::JobResult> &res, std::string &err) -> int {
         const long long c = ++calls;
         if (fail_every > 0 && jobs.size() > 2 && c % fail_every == 0) { err = "stand-in device: injected batch failure"; return -2; }
-        res.assign(jobs.size(), barb200::JobResult());
-        for (size_t j = 0; j < jobs.size(); ++j) {
-            HtParams q = *hp; q.progressive = jobs[j].progressive;
-            int64_t nw = 0; int status = 0, sum = 0;
-            for (int i = 0; i < jobs[j].n_seq; ++i) sum += jobs[j].lens[i];
-            for (int b = 0; b < sum; ++b) if (jobs[j].seqs[b] > 4) { err = "sequence code > 4"; return -3; }      // what the device rejects too
-            int64_t *w = hosttest_poa_msa_trace(&q, jobs[j].n_seq, jobs[j].lens, jobs[j].seqs, &nw, &status);
-            if (status) { free(w); err = "stand-in device: job failed"; return -5; }
-            const int ml = (int)w[1];
-            const size_t nb = (size_t)jobs[j].n_seq * ml, nwm = (nb + 7) / 8;
-            res[j].msa.assign((const uint8_t *)(w + (nw - (int64_t)nwm)), (const uint8_t *)(w + (nw - (int64_t)nwm)) + nb);
-            res[j].msa_len = ml; res[j].cells = w[2];
-            free(w);
-        }
-        return 0;
+        return hosttest_device_batch(*hp, 0, jobs, res, err);
     };
     barb200::EndQueue q(n_lanes, exec, max_jobs, 1e18);
     // flat -> per-flower pointer tables
@@ -508,4 +523,61 @@ extern "C" double hosttest_lane_budget_bytes(double free_b, double total_b, doub
 }
 extern "C" double hosttest_retry_plane_scale(double budget, double fixed_bytes, double plane_bytes) {
     return barb200::retry_plane_scale(budget, fixed_bytes, plane_bytes);
+}
+
+// ---- the plan of a stage (stage_plan.h) ----
+static int plan_error(const std::string &e, int rc, char *err, int err_len) { snprintf(err, err_len, "%s", e.c_str()); return rc; }
+
+// A stage of n jobs (caller order; lengths and bases back to back) under Cactus' band and `threads_per_block`, sized for (grow,
+// worst_case); with per_sm > 0 also fitted to per_sm CTAs per SM of every class on sm_count SMs within `budget` bytes. Out: cost[n]
+// in caller order; perm, msa_off, msa_stride [n] in internal order; buckets[6 x 6] = threads, job_base, n_jobs, slots, plane ints
+// per slot, slot bytes. Returns the number of buckets, or the BARB200_* code of a rejection with its message in err.
+extern "C" int hosttest_stage_plan(int64_t n, const int *n_seq, const int *lens, const uint8_t *seqs, int threads_per_block, double grow, int worst_case,
+                                   int per_sm, int sm_count, double budget, double *cost, int64_t *perm, int64_t *msa_off, int64_t *msa_stride,
+                                   int64_t *buckets, char *err, int err_len) {
+    barb200_params p;
+    params_default(&p);
+    p.threads_per_block = threads_per_block;
+    JobTable T;
+    std::string e = table_of_arrays(p, 4, n, n_seq, lens, seqs, nullptr, T);
+    if (!e.empty()) return plan_error(e, BARB200_EINVAL, err, err_len);
+    StagePlan S = plan_stage_order(T, all_jobs(n), p, grow, worst_case != 0, sm_count, true);
+    if (per_sm > 0 && !(e = fit_stage(S, std::vector<int>(S.buckets.size(), per_sm), sm_count, budget)).empty()) return plan_error(e, BARB200_ENOMEM, err, err_len);
+    for (int64_t j = 0; j < n; ++j) { cost[j] = T.jobs[j].cost; perm[j] = S.perm[j]; msa_off[j] = S.desc[j].msa_off; msa_stride[j] = S.desc[j].msa_stride; }
+    for (size_t b = 0; b < S.buckets.size(); ++b) {
+        const PlanBucket &B = S.buckets[b];
+        const int64_t v[6] = {B.T, B.job_base, B.n_jobs, B.slots, B.lay.plane_cap, B.lay.slot_bytes};
+        memcpy(buckets + 6 * b, v, sizeof(v));
+    }
+    return (int)S.buckets.size();
+}
+// The capacity retry after a round of a stage over the caller's jobs perm[n], sized for (grow, worst_case) with plane_cap ints of
+// planes per slot, whose jobs ended with status[n]: 0 with redo[*n_redo] and the next (grow, worst_case), or BARB200_EJOB and err.
+extern "C" int hosttest_retry_round(int64_t n, const int *status, const int64_t *perm, double grow, int worst_case, int64_t plane_cap, int64_t *redo,
+                                    int64_t *n_redo, double *next_grow, int *next_worst, char *err, int err_len) {
+    StagePlan S;
+    S.grow = grow; S.worst_case = worst_case != 0; S.perm.assign(perm, perm + n);
+    S.buckets.resize(1); S.buckets[0].lay.plane_cap = plane_cap;
+    RetryRound next;
+    const std::string e = retry_round(S, std::vector<int>(status, status + n), next);
+    if (!e.empty()) return plan_error(e, BARB200_EJOB, err, err_len);
+    *n_redo = (int64_t)next.jobs.size(); std::copy(next.jobs.begin(), next.jobs.end(), redo);
+    *next_grow = next.grow; *next_worst = next.worst_case;
+    return 0;
+}
+// where the device batches of n jobs of sum_len[n] bases end; returns their number
+extern "C" int64_t hosttest_chunk_ends(int64_t n, const int64_t *sum_len, int64_t *ends) {
+    JobTable T;
+    T.jobs.resize(n);
+    for (int64_t j = 0; j < n; ++j) T.jobs[j].sum_len = sum_len[j];
+    const std::vector<size_t> e = chunk_ends(T, all_jobs(n));
+    std::copy(e.begin(), e.end(), ends);
+    return (int64_t)e.size();
+}
+// n jobs of cost[n] dealt over ndev devices: counts[ndev] and every device's share back to back in jobs[n]
+extern "C" void hosttest_deal_jobs(int64_t n, const double *cost, int ndev, int64_t *counts, int64_t *jobs) {
+    JobTable T;
+    T.jobs.resize(n);
+    for (int64_t j = 0; j < n; ++j) T.jobs[j].cost = cost[j];
+    for (const std::vector<int64_t> &s : deal_jobs(T, ndev)) { *counts++ = (int64_t)s.size(); jobs = std::copy(s.begin(), s.end(), jobs); }
 }
