@@ -4,8 +4,8 @@ Python mirror of the reference's POA entry points (bar/inc/poaBarAligner.h) on t
 ``libbarb200.so`` (include/barb200.h). The library is CUDA-only: importing works anywhere, but creating an
 :class:`Engine` without a CUDA device (or without the built library) raises -- there is no CPU fallback.
 """
-from .api import (Engine, Msa, BarB200Error, PoaParams, PairwiseAlignmentParameters, load_library, library_path,
+from .api import (Engine, Msa, BarB200Error, PoaParams, PairwiseAlignmentParameters, MumParams, load_library, library_path,
                   msa_to_base, msa_to_byte, pecan_band, pecan_split_points)
 
-__all__ = ["Engine", "Msa", "BarB200Error", "PoaParams", "PairwiseAlignmentParameters", "load_library", "library_path",
+__all__ = ["Engine", "Msa", "BarB200Error", "PoaParams", "PairwiseAlignmentParameters", "MumParams", "load_library", "library_path",
            "msa_to_base", "msa_to_byte", "pecan_band", "pecan_split_points"]

@@ -44,6 +44,10 @@ class _CPecanParams(C.Structure):
                 ("dynamic_anchor_expansion", C.c_int)]
 
 
+class _CMumParams(C.Structure):
+    _fields_ = [("k", C.c_int64), ("u", C.c_int64), ("anchor_matrix_bigger_than_this", C.c_int64), ("recursive_mums", C.c_int)]
+
+
 class _CMsa(C.Structure):
     _fields_ = [("seq_no", C.c_int64), ("column_no", C.c_int64), ("seq_lens", C.POINTER(C.c_int)),
                 ("msa", C.POINTER(C.c_uint8))]
@@ -131,6 +135,13 @@ def load_library():
     lib.barb200_pecan_band.restype = ci
     lib.barb200_pecan_split_points.argtypes = [i64, i64, vp, i64, i64, ci, ci, C.POINTER(vp)]
     lib.barb200_pecan_split_points.restype = i64
+    mp = C.POINTER(_CMumParams)
+    lib.barb200_mum_params_default.argtypes = [mp]
+    lib.barb200_mum_params_default.restype = None
+    lib.barb200_pecan_anchor_pairs_batch.argtypes = [vp, mp, i64, vp, vp, vp, vp, vp, vp]
+    lib.barb200_pecan_anchor_pairs_batch.restype = ci
+    lib.barb200_mum_last_timing.argtypes = [vp]
+    lib.barb200_mum_last_timing.restype = ci
     _LIB = lib
     return lib
 
@@ -199,6 +210,15 @@ class PairwiseAlignmentParameters:
                  splitMatrixBiggerThanThis=3000, dynamicAnchorExpansion=0):
         self.c = _CPecanParams(threshold, minDiagsBetweenTraceBack, traceBackDiagonals, diagonalExpansion,
                                int(splitMatrixBiggerThanThis) * int(splitMatrixBiggerThanThis), dynamicAnchorExpansion)
+
+
+class MumParams:
+    """The PairwiseAlignmentParameters fields MUM anchoring reads (getAnchorPairsForPairwiseAlignmentParameters,
+    submodules/cPecan/impl/pairwiseAligner.c:1222-1231; the <bar><pecan> keys of bar/impl/bar.c:25-33):
+    anchorMatrixBiggerThanThis is the XML side length, squared here as bar.c:26 does."""
+
+    def __init__(self, k=50, u=1, anchorMatrixBiggerThanThis=500, recursiveMums=1):
+        self.c = _CMumParams(k, u, int(anchorMatrixBiggerThanThis) * int(anchorMatrixBiggerThanThis), recursiveMums)
 
 
 class _PairTable:
@@ -458,6 +478,30 @@ class Engine:
         """single-pair form with the reference's argument order; returns the (score, x, y) triples"""
         return self.get_aligned_pairs_using_anchors_batch(
             [(sX, sY, anchorPairs, alignmentHasRaggedLeftEnd, alignmentHasRaggedRightEnd)], params)[0][0]
+
+    def mum_anchor_pairs_batch(self, pairs, params=None):
+        """getAnchorPairsForPairwiseAlignmentParameters with MUM anchors for many sequence pairs on the device.
+        pairs: list of (sX, sY, ...) (further items are ignored). Returns per pair an int64 [n, 2] array of (x, y) anchors in the
+        reference's order."""
+        params = params or MumParams()
+        t = pairs if isinstance(pairs, _PairTable) else _PairTable(pairs)
+        m = max(t.n, 1)
+        out = (C.c_void_p * m)()
+        n_out = np.zeros(m, np.int64)
+        self._check(self.lib.barb200_pecan_anchor_pairs_batch(self.ctx, C.byref(params.c), t.n, t.sx, t.lx.ctypes.data, t.sy,
+                                                              t.ly.ctypes.data, out, n_out.ctypes.data))
+        res = []
+        for i in range(t.n):
+            k = int(n_out[i])
+            res.append(np.ctypeslib.as_array(C.cast(out[i], C.POINTER(C.c_int64)), shape=(max(2 * k, 1),))[: 2 * k].reshape(k, 2).copy())
+            self.lib.barb200_free(out[i])
+        return res
+
+    def mum_last_timing(self):
+        """the calling thread's last mum_anchor_pairs_batch: dict(kernel_ms, wall_ms, launches)"""
+        out = np.zeros(3)
+        self._check(self.lib.barb200_mum_last_timing(out.ctypes.data))
+        return dict(kernel_ms=float(out[0]), wall_ms=float(out[1]), launches=int(out[2]))
 
     def pecan_stage(self, pairs, params=None):
         params = params or PairwiseAlignmentParameters()

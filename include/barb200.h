@@ -190,6 +190,30 @@ int64_t barb200_pecan_split_points(int64_t lx, int64_t ly, const int64_t *anchor
                                    int64_t **splits_out);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * cPecan mode's anchors: the MUM chains of getAnchorPairsForPairwiseAlignmentParameters with useMumAnchors = 1
+ * (submodules/cPecan/impl/pairwiseAligner.c:1222-1231 -> getAlignedMums :1849-2121), which addMultipleAlignedPairs computes
+ * for every sequence pair before its posteriors (getAlignedPairs :1527-1534).
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int64_t k;                              /* 50; k-mer length, 1..64 */
+    int64_t u;                              /* 1; a match must be longer than u + either neighbour's in Y's k-mer order */
+    int64_t anchor_matrix_bigger_than_this; /* 500*500; <bar><pecan anchorMatrixBiggerThanThis> SQUARED as bar.c:25-26 does */
+    int recursive_mums;                     /* 1; one non-recursive level into every gap of the chain larger than the above */
+} barb200_mum_params;
+void barb200_mum_params_default(barb200_mum_params *p);
+
+/* For pair i: NUL-free 7-bit ASCII strings sx[i] (length lx[i]) and sy[i] (ly[i]). anchors_out[i] = malloc'd n_anchor_out[i] x 2
+ * int64 (x, y), 0-based, in the reference's order -- strictly increasing in both with recursive_mums (what
+ * barb200_pecan_aligned_pairs_batch takes), last MUM first and each MUM backwards without. Release with barb200_free.
+ * BARB200_EINVAL for k outside 1..64, u < 0, or a NUL / non-ASCII byte. */
+int barb200_pecan_anchor_pairs_batch(barb200_ctx *ctx, const barb200_mum_params *p, int64_t n_pairs,
+                                     const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
+                                     int64_t **anchors_out, int64_t *n_anchor_out);
+/* The calling thread's last barb200_pecan_anchor_pairs_batch: out[0] device time of its kernels and copies (ms), out[1] wall
+ * time of the call (ms), out[2] kernels launched. For reports. */
+int barb200_mum_last_timing(double out[3]);
+
+/* ------------------------------------------------------------------------------------------------------------
  * The end queue, asynchronously. barb200_flower_submit takes the arguments of make_consistent_partial_order_alignments
  * (bar/inc/poaBarAligner.h:108; right_end_indexes == NULL: independent ends, no cross-end trimming -- the single-end case of
  * make_flower_alignment_poa, poaBarAligner.c:1119-1143), copies what it needs and returns at once; the strings may be released

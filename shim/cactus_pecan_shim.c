@@ -14,8 +14,9 @@
  *        (this is the call makeAlignmentUsingAllPairs issues, multipleAligner.c:690, i.e. what makeAlignment does
  *        whenever spanningTrees * (n-1) >= n(n-1)/2, :893-895).
  *
- * Anchors stay the reference's code (getAnchorPairsForPairwiseAlignmentParameters, pairwiseAligner.c:1222-1233: MUM
- * chains on the host), and so does everything above: makeAlignment's pair selection, the poset alignment, endAligner.c,
+ * Anchors of a round of pairs: with useMumAnchors (Cactus' default) one barb200_pecan_anchor_pairs_batch call, the device's
+ * restatement of getAnchorPairsForPairwiseAlignmentParameters (pairwiseAligner.c:1222-1231: MUM chains); otherwise (the lastz
+ * path) the reference's own code on the host. Everything above stays the reference's: makeAlignment's pair selection, the poset alignment, endAligner.c,
  * flowerAligner.c, bar(). The state machine must be the reference's five-state machine with its built-in constants
  * (stateMachine5_construct(fiveState), the one bar() builds at bar/impl/bar.c:66); anything else aborts.
  *
@@ -176,19 +177,37 @@ static void align_pair_list(StateMachine *sM, stList *seqFrags, const int64_t *f
     int64_t *lx = st_malloc(8 * pairNo), *ly = st_malloc(8 * pairNo), *na = st_malloc(8 * pairNo), *nOut = st_malloc(8 * pairNo);
     int64_t **anchors = st_malloc(sizeof(int64_t *) * pairNo), **trip = st_malloc(sizeof(int64_t *) * pairNo);
     uint8_t *rl = st_malloc(pairNo), *rr = st_malloc(pairNo);
-    /* anchors: the reference's host code (getAlignedPairs, pairwiseAligner.c:1527-1534), one pair per thread -- the reference
-     * itself runs it concurrently from bar()'s OpenMP loop over ends (bar/impl/bar.c:90-94) */
-#if defined(_OPENMP)
-#pragma omp parallel for schedule(dynamic, 1)
-#endif
     for (int64_t i = 0; i < pairNo; i++) {
         SeqFrag *f1 = stList_get(seqFrags, first[i]), *f2 = stList_get(seqFrags, second[i]);
         sx[i] = f1->seq; sy[i] = f2->seq; lx[i] = strlen(f1->seq); ly[i] = strlen(f2->seq);
-        stList *anchorPairs = getAnchorPairsForPairwiseAlignmentParameters(f1->seq, f2->seq, lx[i], ly[i], p);
-        anchors[i] = flatten_anchors(anchorPairs, &na[i]);
-        stList_destruct(anchorPairs);
         rl[i] = f1->leftEndId != f2->leftEndId;                /* addMultipleAlignedPairs, multipleAligner.c:660-661 */
         rr[i] = f1->rightEndId != f2->rightEndId;
+    }
+    /* anchors (getAlignedPairs, pairwiseAligner.c:1527-1534): MUM chains of the whole round in one device batch. A pair with
+     * lX * lY <= anchorMatrixBiggerThanThis has no anchors (:1224-1226), so a round of such pairs (short ends, the common case)
+     * makes no anchor call at all. */
+    if (p->useMumAnchors) {
+        int64_t searched = 0;
+        for (int64_t i = 0; i < pairNo; i++) {
+            anchors[i] = NULL; na[i] = 0;
+            searched += lx[i] * ly[i] > p->anchorMatrixBiggerThanThis;
+        }
+        barb200_mum_params mp;
+        mp.k = p->k; mp.u = p->u; mp.anchor_matrix_bigger_than_this = p->anchorMatrixBiggerThanThis; mp.recursive_mums = (int)p->recursiveMums;
+        if (searched > 0 && barb200_pecan_anchor_pairs_batch(ctx, &mp, pairNo, sx, lx, sy, ly, anchors, na) != BARB200_OK) {
+            st_errAbort("barb200: MUM anchor batch failed: %s", barb200_last_error(ctx));
+        }
+    } else {
+        /* the lastz path: the reference's host code, one pair per thread -- the reference itself runs it concurrently from
+         * bar()'s OpenMP loop over ends (bar/impl/bar.c:90-94) */
+#if defined(_OPENMP)
+#pragma omp parallel for schedule(dynamic, 1)
+#endif
+        for (int64_t i = 0; i < pairNo; i++) {
+            stList *anchorPairs = getAnchorPairsForPairwiseAlignmentParameters(sx[i], sy[i], lx[i], ly[i], p);
+            anchors[i] = flatten_anchors(anchorPairs, &na[i]);
+            stList_destruct(anchorPairs);
+        }
     }
     if (barb200_pecan_aligned_pairs_batch(ctx, &q, pairNo, sx, lx, sy, ly, (const int64_t *const *) anchors, na, rl, rr, trip, nOut, NULL, NULL) != BARB200_OK) {
         st_errAbort("barb200: pair-HMM batch failed: %s", barb200_last_error(ctx));
@@ -214,7 +233,7 @@ static void align_pair_list(StateMachine *sM, stList *seqFrags, const int64_t *f
         stList_destruct(alignedPairs);
         stList_append(scores, stIntTuple_construct3(distance, first[k], second[k]));
         barb200_free(trip[k]);
-        free(anchors[k]);
+        free(anchors[k]);                                  /* malloc'd by either path (barb200_free is free), or NULL */
     }
     free(sx); free(sy); free(lx); free(ly); free(na); free(nOut); free(anchors); free(trip); free(rl); free(rr);
 }
