@@ -20,14 +20,6 @@
 #include <stdint.h>
 #include "poa_types.h"
 
-#if defined(__CUDA_ARCH__)
-#define GT_THREADS(tid, T) for (int tid = (int)threadIdx.x, _gt_once = 1; _gt_once; _gt_once = 0)
-#define GT_SYNC() __syncthreads()
-#else
-#define GT_THREADS(tid, T) for (int tid = 0; tid < (T); ++tid)
-#define GT_SYNC() ((void)0)
-#endif
-
 namespace barb200 {
 
 struct GuideTreeParams { int k, w; };        // partialOrderAlignmentMinimizerK / W

@@ -15,48 +15,9 @@
 #pragma once
 #include <cuda_runtime.h>
 #include "poa_graph.cuh"
+#include "graph_phases.cuh"
 
 namespace barb200 {
-
-// exclusive prefix sum of a[0..n) in place (global or shared memory); returns the total. All threads of the CTA.
-// ws: >= 32 ints of shared memory.
-__device__ int cta_excl_scan(int *a, int n, int *ws) {
-    const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = T >> 5;
-    const int chunk = (n + T - 1) / T, b = min(n, tid * chunk), e = min(n, b + chunk);
-    int s = 0;
-    for (int i = b; i < e; ++i) s += a[i];
-    int inc = s;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) { const int v = __shfl_up_sync(0xffffffffu, inc, off); if (lane >= off) inc += v; }
-    __syncthreads();                       // ws may still be read by a previous call
-    if (lane == 31) ws[warp] = inc;
-    __syncthreads();
-    int woff = 0, total = 0;
-    for (int k = 0; k < nw; ++k) { const int v = ws[k]; if (k < warp) woff += v; total += v; }
-    int run = woff + inc - s;
-    for (int i = b; i < e; ++i) { const int v = a[i]; a[i] = run; run += v; }
-    __syncthreads();
-    return total;
-}
-
-// inclusive prefix maximum of a[0..n) in place. All threads of the CTA. ws: >= 32 ints of shared memory.
-__device__ void cta_incl_max_scan(int *a, int n, int *ws) {
-    const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = T >> 5;
-    const int chunk = (n + T - 1) / T, b = min(n, tid * chunk), e = min(n, b + chunk);
-    int s = INT32_MIN;
-    for (int i = b; i < e; ++i) s = max(s, a[i]);
-    int inc = s;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) { const int v = __shfl_up_sync(0xffffffffu, inc, off); if (lane >= off) inc = max(inc, v); }
-    int run = __shfl_up_sync(0xffffffffu, inc, 1);
-    if (lane == 0) run = INT32_MIN;
-    __syncthreads();
-    if (lane == 31) ws[warp] = inc;
-    __syncthreads();
-    for (int k = 0; k < nw; ++k) if (k < warp) run = max(run, ws[k]);
-    for (int i = b; i < e; ++i) { run = max(run, a[i]); a[i] = run; }
-    __syncthreads();
-}
 
 // ---- edge lists with atomic pool allocation (same lists as graph_add_edge; chunk placement in the pool differs) ----
 __device__ __forceinline__ bool grow_in_par(Graph &g, int t) {
@@ -123,7 +84,9 @@ __device__ void cta_add_first_sequence(Graph &g, const uint8_t *seq, int len, in
 
 // abpoa_add_subgraph_alignment(SRC, SINK, inc_both_ends = 1), abpoa_graph.c:689-774. All threads.
 // Scratch: g.tmp0[q] = node that query base q ends up on, g.tmp1[q] = 1 if that node is new. ws: >= 32 ints shared.
-__device__ void cta_fuse_alignment(Graph &g, const uint8_t *seq, int L, const uint64_t *cigar, int n_cigar, int read_id, int *ws) {
+// scr / scr_bytes: dynamic shared memory for the order splice (graph_phases.cuh), unused by the caller meanwhile.
+__device__ void cta_fuse_alignment(Graph &g, const uint8_t *seq, int L, const uint64_t *cigar, int n_cigar, int read_id, int *ws,
+                                   unsigned char *scr, int scr_bytes) {
     const int tid = threadIdx.x, T = blockDim.x;
     if (n_cigar == 0) return;
     int *node_of = g.tmp0, *is_new = g.tmp1;
@@ -170,7 +133,9 @@ __device__ void cta_fuse_alignment(Graph &g, const uint8_t *seq, int L, const ui
     // fusions rely on when they move a path onto an aligned sibling), an inserted new node opens a block right after
     // the block of the previous path node. Anchors are non-decreasing along the path, so the new node with rank m
     // (in query order) and anchor A lands at A + 1 + m, and old index i moves up by the number of anchors < i.
-    {
+    // In the shared-memory scratch where it fits (graph_phases.cuh: splice_order_smem), else on global scratch arrays.
+    if (splice_smem_fits(L, first_new, first_new + n_new, scr_bytes)) splice_order_smem(g, node_of, L, first_new, n_new, scr, ws, T);
+    else {
         int *anc = g.remain, *cnt = g.msa_rank, *new_i2n = g.tmp1;
         const int n_old = first_new;
         for (int q = tid; q < L; q += T) {
@@ -436,9 +401,11 @@ __device__ void bfs_index_smem(Graph &g, const BfsScratch &B) {      // one thre
 
 // All threads. scr/scr_bytes: dynamic shared memory scratch; ws: >= 32 ints shared.
 // have_order: index_to_node / node_to_index already hold a valid topological order (cta_fuse_alignment keeps it up to
-// date), so only the edge sort, max_remain and the row tables are (re)built.
+// date), so only the edge sort, max_remain and the row tables are (re)built: in the shared-memory scratch where the graph fits
+// (graph_phases.cuh: topo_rows_smem), else by the global-memory form below.
 __device__ void cta_topo_sort(Graph &g, RowTables &rt, unsigned char *scr, int scr_bytes, int *ws, bool have_order) {
     const int tid = threadIdx.x, T = blockDim.x, n = g.node_n;
+    if (have_order && topo_smem_fits(n, scr_bytes)) { topo_rows_smem(g, rt, scr, ws, T); return; }
     if (have_order) {
         for (int v = tid; v < n; v += T) graph_sort_node_edges(g, v);
         __syncthreads();

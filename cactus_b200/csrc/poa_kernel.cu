@@ -502,7 +502,7 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
                 PHASE_TICK(PH_BACKTRACK);
                 __syncthreads();
                 if (A.serial_phases) { if (tid == 0 && !S.g.err) graph_fuse_alignment(S.g, q, S.d.cigar, S.d.n_cigar, read); }
-                else if (!S.g.err) cta_fuse_alignment(S.g, q, L, S.d.cigar, S.d.n_cigar, read, ws);
+                else if (!S.g.err) cta_fuse_alignment(S.g, q, L, S.d.cigar, S.d.n_cigar, read, ws, dyn_smem, A.scratch_bytes);
                 PHASE_TICK(PH_FUSE);
             }
             __syncthreads();

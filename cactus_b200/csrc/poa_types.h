@@ -13,6 +13,17 @@
 #define HD inline
 #endif
 
+// The threads of a CTA program written once for both targets (guide_tree.cuh, graph_phases.cuh): on the device every thread runs
+// the body once with its own tid; on the host (tests/hosttest) the body runs for tid = 0 .. T-1 one after the other, and the barrier
+// between two such loops is the loop's end.
+#if defined(__CUDA_ARCH__)
+#define GT_THREADS(tid, T) for (int tid = (int)threadIdx.x, _gt_once = 1; _gt_once; _gt_once = 0)
+#define GT_SYNC() __syncthreads()
+#else
+#define GT_THREADS(tid, T) for (int tid = 0; tid < (T); ++tid)
+#define GT_SYNC() ((void)0)
+#endif
+
 namespace barb200 {
 
 constexpr int SRC_ID = 0;    // ABPOA_SRC_NODE_ID  (abPOA include/abpoa.h:27)
