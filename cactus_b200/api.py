@@ -142,6 +142,8 @@ def load_library():
     lib.barb200_pecan_anchor_pairs_batch.restype = ci
     lib.barb200_mum_last_timing.argtypes = [vp]
     lib.barb200_mum_last_timing.restype = ci
+    lib.barb200_pecan_device_stats.argtypes = [vp, vp, vp, ci]
+    lib.barb200_pecan_device_stats.restype = ci
     _LIB = lib
     return lib
 
@@ -497,8 +499,20 @@ class Engine:
             self.lib.barb200_free(out[i])
         return res
 
+    def pecan_device_stats(self):
+        """per device of the context, the sequence pairs the batch calls have run there since the context was created:
+        dict(hmm_pairs=[...] (get_aligned_pairs_using_anchors_batch), mum_pairs=[...] (mum_anchor_pairs_batch, only pairs that
+        needed the device)); the staged form is not counted"""
+        n = self.device_count()
+        hmm, mum = np.zeros(max(n, 1), np.int64), np.zeros(max(n, 1), np.int64)
+        rc = self.lib.barb200_pecan_device_stats(self.ctx, hmm.ctypes.data, mum.ctypes.data, n)
+        if rc < 0:
+            self._check(rc)
+        return dict(hmm_pairs=[int(v) for v in hmm[:n]], mum_pairs=[int(v) for v in mum[:n]])
+
     def mum_last_timing(self):
-        """the calling thread's last mum_anchor_pairs_batch: dict(kernel_ms, wall_ms, launches)"""
+        """the calling thread's last mum_anchor_pairs_batch: dict(kernel_ms (with several devices: the slowest device's),
+        wall_ms, launches (all devices))"""
         out = np.zeros(3)
         self._check(self.lib.barb200_mum_last_timing(out.ctypes.data))
         return dict(kernel_ms=float(out[0]), wall_ms=float(out[1]), launches=int(out[2]))

@@ -127,8 +127,10 @@ int host_threads(barb200_ctx *ctx) {
     return std::max(1, n / std::max(1, tl_thread_divisor));
 }
 int default_progressive(barb200_ctx *ctx) { return ctx->p.progressive_poa; }
-int ctx_device(barb200_ctx *ctx) { return ctx->devs[0]->ordinal; }
-int ctx_sm_count(barb200_ctx *ctx) { return ctx->devs[0]->sm_count; }
+void set_host_thread_share(int n) { tl_thread_divisor = std::max(1, n); }
+int ctx_device_count(barb200_ctx *ctx) { return (int)ctx->devs.size(); }
+int ctx_device(barb200_ctx *ctx, int dev) { return ctx->devs[dev]->ordinal; }
+int ctx_sm_count(barb200_ctx *ctx, int dev) { return ctx->devs[dev]->sm_count; }
 double ctx_mem_fraction(barb200_ctx *ctx) { return ctx->p.mem_fraction > 0 ? ctx->p.mem_fraction : 0.85; }
 int total_lanes(barb200_ctx *ctx) { return (int)ctx->devs.size() * ctx->lanes_per_device; }
 void **dispatcher_slot(barb200_ctx *ctx) { return &ctx->dispatcher; }
@@ -199,10 +201,10 @@ static void dev_free(Device &D, void *p, size_t bytes) {
 }
 
 namespace barb200 {
-int device_alloc(barb200_ctx *ctx, void **p, size_t bytes) { return dev_alloc(*ctx->devs[0], p, bytes) == cudaSuccess ? 0 : -1; }
-void device_free(barb200_ctx *ctx, void *p, size_t bytes) { dev_free(*ctx->devs[0], p, bytes); }
-void *pinned_take(barb200_ctx *ctx, size_t bytes, size_t *got) { return ::pinned_take(*ctx->devs[0], bytes, got); }
-void pinned_give(barb200_ctx *ctx, void *p, size_t bytes) { ::pinned_give(*ctx->devs[0], p, bytes); }
+int device_alloc(barb200_ctx *ctx, int dev, void **p, size_t bytes) { return dev_alloc(*ctx->devs[dev], p, bytes) == cudaSuccess ? 0 : -1; }
+void device_free(barb200_ctx *ctx, int dev, void *p, size_t bytes) { dev_free(*ctx->devs[dev], p, bytes); }
+void *pinned_take(barb200_ctx *ctx, int dev, size_t bytes, size_t *got) { return ::pinned_take(*ctx->devs[dev], bytes, got); }
+void pinned_give(barb200_ctx *ctx, int dev, void *p, size_t bytes) { ::pinned_give(*ctx->devs[dev], p, bytes); }
 }  // namespace barb200
 
 extern "C" void barb200_params_default(barb200_params *p) { params_default(p); }

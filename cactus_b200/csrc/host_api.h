@@ -55,20 +55,24 @@ void set_error(barb200_ctx *ctx, const std::string &msg);
 std::string get_error(barb200_ctx *ctx);
 int host_threads(barb200_ctx *ctx);
 int default_progressive(barb200_ctx *ctx);
-// context facts for pecan.cu, which runs the pair-HMM work on the context's first device
-int ctx_device(barb200_ctx *ctx);
-int ctx_sm_count(barb200_ctx *ctx);
+// context facts for pecan.cu and mum_anchor.cu, which run cPecan mode's work on the context's devices 0 .. ctx_device_count - 1
+int ctx_device_count(barb200_ctx *ctx);
+int ctx_device(barb200_ctx *ctx, int dev);     // the CUDA ordinal of the context's device `dev`
+int ctx_sm_count(barb200_ctx *ctx, int dev);
 double ctx_mem_fraction(barb200_ctx *ctx);
-// device blocks from the first device's grow-only cache (cudaMalloc / cudaFree per call cost milliseconds); 0 on success
-int device_alloc(barb200_ctx *ctx, void **p, size_t bytes);
-void device_free(barb200_ctx *ctx, void *p, size_t bytes);
-// pinned host blocks from the first device's pool (pinned_take: nullptr if cudaMallocHost fails; *got = the block's size)
-void *pinned_take(barb200_ctx *ctx, size_t bytes, size_t *got);
-void pinned_give(barb200_ctx *ctx, void *p, size_t bytes);
-// pecan.cu: the context's pair-HMM state (streams, ring scratch, batch group commit), made by barb200_create on the first device
+// device blocks from device `dev`'s grow-only cache (cudaMalloc / cudaFree per call cost milliseconds); 0 on success
+int device_alloc(barb200_ctx *ctx, int dev, void **p, size_t bytes);
+void device_free(barb200_ctx *ctx, int dev, void *p, size_t bytes);
+// pinned host blocks from device `dev`'s pool (pinned_take: nullptr if cudaMallocHost fails; *got = the block's size)
+void *pinned_take(barb200_ctx *ctx, int dev, size_t bytes, size_t *got);
+void pinned_give(barb200_ctx *ctx, int dev, void *p, size_t bytes);
+// a host thread that runs one device's share of a batch over `n` devices takes 1/n of host_threads() (1: all of them)
+void set_host_thread_share(int n);
+// pecan.cu: the context's pair-HMM state (per device: streams, ring scratch; one batch group commit), made by barb200_create
 void **pecan_slot(barb200_ctx *ctx);
 int pecan_create(barb200_ctx *ctx);            // 0 on success; the slot is set either way, so barb200_destroy cleans up
 void pecan_destroy(barb200_ctx *ctx);
+void pecan_count_mum_pairs(barb200_ctx *ctx, int dev, int64_t n);   // barb200_pecan_device_stats' MUM-anchor count
 
 }  // namespace barb200
 

@@ -13,16 +13,21 @@
 //   mum_chain_kernel ......... the MUM rule, sweep line and traceback of each problem, one thread each (serial in x), with the
 //                              chain copied densely for the host.
 // The host splices the chains and the gaps' chains into the reference's order (mum_plan.h: splice).
+// On a context of several devices the pairs that need a device are dealt to the devices by their bytes, and every device plans
+// and runs its chunks on a host thread of its own (run_devices).
 #include <cuda_runtime.h>
 #include <omp.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <new>
 #include <string>
+#include <thread>
 #include <vector>
 #include "host_api.h"
 #include "mum_anchor.cuh"
+#include "pecan_plan.h"
 
 using namespace barb200;
 using namespace barb200::mum;
@@ -158,6 +163,7 @@ inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 // The device work of one chunk: buffers carved from one cached block, one stream.
 struct Chunk {
     barb200_ctx *ctx;
+    int dev = 0;                   // the context's device the chunk runs on
     cudaStream_t s = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     void *blk = nullptr; size_t blk_bytes = 0;
@@ -170,7 +176,7 @@ struct Chunk {
     int max_words = 1;
     float kernel_ms = 0; int launches = 0;
     ~Chunk() {
-        if (blk) device_free(ctx, blk, blk_bytes);
+        if (blk) device_free(ctx, dev, blk, blk_bytes);
         if (e0) cudaEventDestroy(e0);
         if (e1) cudaEventDestroy(e1);
         if (s) cudaStreamDestroy(s);
@@ -196,8 +202,8 @@ int run_pass(Chunk &C, const std::vector<Problem> &probs, std::vector<std::vecto
     const size_t b_probs = align256(sizeof(Problem) * np), b_tiles = align256(sizeof(Tile) * std::max<size_t>(tiles.size(), 1)),
                  b_off = align256(8 * (size_t)np), b_n = align256(4 * (size_t)np), bytes = b_probs + b_tiles + b_off + b_n + 256;
     void *tb = nullptr;
-    if (device_alloc(ctx, &tb, bytes) != 0) { set_error(ctx, "device allocation failed (MUM pass tables)"); return BARB200_ENOMEM; }
-    struct Free { barb200_ctx *c; void *p; size_t b; ~Free() { device_free(c, p, b); } } fr{ctx, tb, bytes};
+    if (device_alloc(ctx, C.dev, &tb, bytes) != 0) { set_error(ctx, "device allocation failed (MUM pass tables)"); return BARB200_ENOMEM; }
+    struct Free { barb200_ctx *c; int d; void *p; size_t b; ~Free() { device_free(c, d, p, b); } } fr{ctx, C.dev, tb, bytes};
     Problem *d_probs = (Problem *)tb;
     Tile *d_tiles = (Tile *)((char *)tb + b_probs);
     int64_t *d_out_off = (int64_t *)((char *)tb + b_probs + b_tiles);
@@ -206,7 +212,7 @@ int run_pass(Chunk &C, const std::vector<Problem> &probs, std::vector<std::vecto
     CUDA_TRY(ctx, cudaMemcpyAsync(d_probs, probs.data(), sizeof(Problem) * np, cudaMemcpyHostToDevice, C.s));
     if (!tiles.empty()) CUDA_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), sizeof(Tile) * tiles.size(), cudaMemcpyHostToDevice, C.s));
     CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 8, C.s));
-    const int grid = ctx_sm_count(ctx) * 8;
+    const int grid = ctx_sm_count(ctx, C.dev) * 8;
     int32_t *cur = C.d_sa, *other = C.d_sb;
     if (!tiles.empty()) {
         const size_t smem = (size_t)kTile * C.max_words * 8 + (size_t)kTile * 2;
@@ -240,9 +246,9 @@ int run_pass(Chunk &C, const std::vector<Problem> &probs, std::vector<std::vecto
     return BARB200_OK;
 }
 
-int run_chunk(barb200_ctx *ctx, const MumParams &P, int64_t n, const char *const *sx, const int64_t *lx, const char *const *sy,
+int run_chunk(barb200_ctx *ctx, int dev, const MumParams &P, int64_t n, const char *const *sx, const int64_t *lx, const char *const *sy,
               const int64_t *ly, const Alphabet *alpha, int64_t **out, int64_t *n_out, float *kernel_ms, int *launches) {
-    Chunk C; C.ctx = ctx; C.k = (int)P.k; C.u = P.u;
+    Chunk C; C.ctx = ctx; C.dev = dev; C.k = (int)P.k; C.u = P.u;
     // active pairs: lX * lY > anchorMatrixBiggerThanThis (the early return of :1224-1226)
     std::vector<int64_t> act;
     for (int64_t i = 0; i < n; ++i) if (lx[i] * ly[i] > P.bigger) act.push_back(i);
@@ -268,8 +274,8 @@ int run_chunk(barb200_ctx *ctx, const MumParams &P, int64_t n, const char *const
                  b_nx = align256(4 * (size_t)std::max<int64_t>(nx_sum, 1)), b_mums = align256(sizeof(MumRec) * (size_t)std::max<int64_t>(nx_sum, 1)),
                  b_chain = align256(sizeof(ChainMum) * (size_t)std::max<int64_t>(nx_sum, 1));
     C.blk_bytes = b_pairs + b_koff + b_codes + b_keys + 2 * b_ny + 3 * b_nx + b_mums + 2 * b_chain;
-    cudaSetDevice(ctx_device(ctx));
-    if (device_alloc(ctx, &C.blk, C.blk_bytes) != 0) { C.blk = nullptr; set_error(ctx, "device allocation failed (MUM anchors); submit fewer or shorter pairs"); return BARB200_ENOMEM; }
+    cudaSetDevice(ctx_device(ctx, dev));
+    if (device_alloc(ctx, dev, &C.blk, C.blk_bytes) != 0) { C.blk = nullptr; set_error(ctx, "device allocation failed (MUM anchors); submit fewer or shorter pairs"); return BARB200_ENOMEM; }
     char *p = (char *)C.blk;
     C.d_pairs = (PairDev *)p; p += b_pairs;
     C.d_kmer_off = (int64_t *)p; p += b_koff;
@@ -298,7 +304,7 @@ int run_chunk(barb200_ctx *ctx, const MumParams &P, int64_t n, const char *const
     CUDA_TRY(ctx, cudaMemcpyAsync(C.d_kmer_off, kmer_off.data(), 8 * kmer_off.size(), cudaMemcpyHostToDevice, C.s));
     CUDA_TRY(ctx, cudaMemcpyAsync(C.d_codes, hc.data(), (size_t)codes, cudaMemcpyHostToDevice, C.s));
     if (kmer_off.back() > 0) {
-        mum_keys_kernel<<<ctx_sm_count(ctx) * 8, 256, 0, C.s>>>(C.d_pairs, C.n_pairs, C.d_kmer_off, C.d_codes, C.d_keys, C.k);
+        mum_keys_kernel<<<ctx_sm_count(ctx, dev) * 8, 256, 0, C.s>>>(C.d_pairs, C.n_pairs, C.d_kmer_off, C.d_codes, C.d_keys, C.k);
         ++C.launches;
     }
     // pass 1: the pairs
@@ -349,6 +355,69 @@ int run_chunk(barb200_ctx *ctx, const MumParams &P, int64_t n, const char *const
     }
     for (int64_t i = 0; i < n; ++i) if (!out[i]) { out[i] = (int64_t *)malloc(16); if (!out[i]) oom = true; }
     if (oom) { set_error(ctx, "host allocation failed (MUM anchors)"); return BARB200_ENOMEM; }
+    pecan_count_mum_pairs(ctx, dev, (int64_t)act.size());
+    return BARB200_OK;
+}
+
+// The pairs [0, n) on device `dev`: chunks (plan_chunks) under the device's free memory, one after the other. kernel_ms and
+// launches accumulate; out / n_out are filled for every pair, also those below anchorMatrixBiggerThanThis.
+int run_share(barb200_ctx *ctx, int dev, const MumParams &P, int64_t n, const char *const *sx, const int64_t *lx, const char *const *sy,
+              const int64_t *ly, const Alphabet *alpha, const std::vector<int64_t> &bytes, int64_t **out, int64_t *n_out, float *kernel_ms, int *launches) {
+    cudaSetDevice(ctx_device(ctx, dev));
+    size_t free_b = 0, total_b = 0;
+    CUDA_TRY(ctx, cudaMemGetInfo(&free_b, &total_b));
+    const int64_t budget = std::max<int64_t>((int64_t)(0.5 * ctx_mem_fraction(ctx) * (double)free_b), 1 << 20);
+    for (const auto &c : plan_chunks(bytes, budget)) {
+        const int rc = run_chunk(ctx, dev, P, c.second - c.first, sx + c.first, lx + c.first, sy + c.first, ly + c.first, alpha + c.first, out + c.first,
+                                 n_out + c.first, kernel_ms, launches);
+        if (rc) return rc;
+    }
+    return BARB200_OK;
+}
+
+// The pairs that need a device (bytes > 0) dealt over the context's devices by their bytes (deal_pairs), each device's share
+// gathered and run by run_share on a host thread of its own, its anchors put back at the caller's indices; the other pairs get
+// an empty list here. kernel_ms = the longest device's kernel time, launches = all devices' launches.
+int run_devices(barb200_ctx *ctx, int ndev, const MumParams &P, int64_t n, const char *const *sx, const int64_t *lx, const char *const *sy,
+                const int64_t *ly, const Alphabet *alpha, const std::vector<int64_t> &bytes, int64_t **out, int64_t *n_out, float *kernel_ms, int *launches) {
+    std::vector<int64_t> act, act_bytes;
+    for (int64_t i = 0; i < n; ++i) {
+        if (bytes[i] > 0) { act.push_back(i); act_bytes.push_back(bytes[i]); continue; }
+        out[i] = (int64_t *)malloc(16);
+        if (!out[i]) { set_error(ctx, "host allocation failed (MUM anchors)"); return BARB200_ENOMEM; }
+    }
+    const std::vector<std::vector<int64_t>> share = barb200::pecan::deal_pairs(act_bytes, ndev);
+    int active = 0;
+    for (const auto &s : share) active += !s.empty();
+    std::vector<int> rcs(ndev, BARB200_OK), dev_launches(ndev, 0);
+    std::vector<float> dev_ms(ndev, 0.f);
+    std::vector<std::string> errs(ndev);
+    auto run_device = [&](int d) {
+        set_host_thread_share(active);
+        try {
+            const std::vector<int64_t> &mine = share[d];
+            const size_t m = mine.size();
+            std::vector<const char *> dsx(m), dsy(m);
+            std::vector<int64_t> dlx(m), dly(m), db(m), dn(m, 0);
+            std::vector<Alphabet> da(m);
+            std::vector<int64_t *> dout(m, nullptr);
+            for (size_t k = 0; k < m; ++k) {
+                const int64_t i = act[mine[k]];
+                dsx[k] = sx[i]; dsy[k] = sy[i]; dlx[k] = lx[i]; dly[k] = ly[i]; db[k] = bytes[i]; da[k] = alpha[i];
+            }
+            rcs[d] = run_share(ctx, d, P, (int64_t)m, dsx.data(), dlx.data(), dsy.data(), dly.data(), da.data(), db, dout.data(), dn.data(), &dev_ms[d], &dev_launches[d]);
+            if (rcs[d]) errs[d] = get_error(ctx);
+            for (size_t k = 0; k < m; ++k) { out[act[mine[k]]] = dout[k]; n_out[act[mine[k]]] = dn[k]; }
+        } catch (const std::bad_alloc &) { rcs[d] = BARB200_ENOMEM; errs[d] = "host allocation failed (MUM anchors)"; }
+        set_host_thread_share(1);
+    };
+    std::vector<std::thread> th;
+    for (int d = 0; d < ndev; ++d) if (!share[d].empty()) th.emplace_back(run_device, d);
+    for (auto &t : th) t.join();
+    for (int d = 0; d < ndev; ++d) {
+        *kernel_ms = std::max(*kernel_ms, dev_ms[d]); *launches += dev_launches[d];
+    }
+    for (int d = 0; d < ndev; ++d) if (rcs[d]) { set_error(ctx, errs[d]); return rcs[d]; }
     return BARB200_OK;
 }
 
@@ -386,18 +455,11 @@ extern "C" int barb200_pecan_anchor_pairs_batch(barb200_ctx *ctx, const barb200_
         bytes[i] = lx[i] * ly[i] > P.bigger ? pair_bytes(lx[i], ly[i], P.k, alpha[i].words) : 0;
     }
     if (!err.empty()) { set_error(ctx, err); return BARB200_EINVAL; }
-    cudaSetDevice(ctx_device(ctx));
-    size_t free_b = 0, total_b = 0;
-    CUDA_TRY(ctx, cudaMemGetInfo(&free_b, &total_b));
-    const int64_t budget = std::max<int64_t>((int64_t)(0.5 * ctx_mem_fraction(ctx) * (double)free_b), 1 << 20);
     for (int64_t i = 0; i < n_pairs; ++i) { anchors_out[i] = nullptr; n_anchor_out[i] = 0; }
     float kms = 0; int launches = 0;
-    int rc = BARB200_OK;
-    for (const auto &c : plan_chunks(bytes, budget)) {
-        rc = run_chunk(ctx, P, c.second - c.first, sx + c.first, lx + c.first, sy + c.first, ly + c.first, alpha.data() + c.first, anchors_out + c.first,
-                       n_anchor_out + c.first, &kms, &launches);
-        if (rc) break;
-    }
+    const int ndev = ctx_device_count(ctx);
+    const int rc = ndev == 1 ? run_share(ctx, 0, P, n_pairs, sx, lx, sy, ly, alpha.data(), bytes, anchors_out, n_anchor_out, &kms, &launches)
+                             : run_devices(ctx, ndev, P, n_pairs, sx, lx, sy, ly, alpha.data(), bytes, anchors_out, n_anchor_out, &kms, &launches);
     if (rc) {
         for (int64_t i = 0; i < n_pairs; ++i) { free(anchors_out[i]); anchors_out[i] = nullptr; n_anchor_out[i] = 0; }
         return rc;

@@ -7,11 +7,14 @@
 // diagonal has <= 96 cells run in 32-thread blocks (24 per SM), all others in 128-thread blocks (6 per SM) whose diagonal
 // ring keeps 320 positions in shared memory and spills the flanks of wider diagonals to an HBM/L2 overflow block (a per-job
 // shift centres the band on the shared part, pecan_cta.cuh). The two launches run concurrently on their own streams.
-// Each resident block owns a slot of the context's ring scratch in HBM (PecanContext: rings, streams, one run at a time) for
+// Each resident block owns a slot of its device's ring scratch in HBM (PecanContext: rings, streams, one run at a time) for
 // the forward MATCH ring, the ring of complete forward cells and the overflow. Candidate pairs (x, y, log posterior) are
 // appended by the kernel, put into the reference's order of emission on the host, compacted on the device, copied back once
 // and finished on the host with libm's exp (the same function the reference calls), threshold and floor. No CPU fallback:
 // the DP only exists as the CUDA kernel below.
+// Every device of the context has its own PecanContext. The batch call on a context of several devices deals whole pairs to
+// the devices by their planned cells and runs each device's share on a host thread of its own (pecan_batch_devices); the
+// staged form runs on the context's first device.
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <math.h>
@@ -20,8 +23,12 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <atomic>
+#include <memory>
 #include <mutex>
+#include <new>
 #include <string>
+#include <thread>
 #include <vector>
 #include "host_api.h"
 #include "batch_merge.h"
@@ -101,59 +108,81 @@ struct Class { int max_w, threads, ctas_per_sm, rws; };
 static const Class kClass[] = {{96, 32, 24, 96}, {INT_MAX, 128, 6, 320}};
 static const int kNumClasses = 2;
 
-// The pair-HMM state of a context (pecan_create). `mu` is held by every use of the device below -- a stage's upload, run and
-// collect, and a batch chunk from create to collect -- so one run at a time owns the streams, the events and the ring scratch.
+// The pair-HMM state of one device of a context (pecan_create). `mu` is held by every use of the device below -- a stage's
+// upload, run and collect, and a batch chunk from create to collect -- so one run at a time owns the streams, the events and
+// the ring scratch.
 struct PecanContext {
-    GroupCommit<PecanRequest> group;             // concurrent barb200_pecan_aligned_pairs_batch callers share device batches
     std::mutex mu;
     double *scratch = nullptr; size_t scratch_bytes = 0;   // grow-only rings (tens of GB: cudaMalloc of that size costs ~0.2 s)
     cudaStream_t stream = nullptr, cls[kNumClasses] = {};
     cudaEvent_t done[kNumClasses] = {}, ev0 = nullptr, ev1 = nullptr;
+    std::atomic<int64_t> hmm_pairs{0}, mum_pairs{0};      // pairs the batch calls ran here (barb200_pecan_device_stats)
 };
-static PecanContext &pecan_of(barb200_ctx *ctx) { return *(PecanContext *)*pecan_slot(ctx); }
+// The context's cPecan state: one PecanContext per device, and one queue for concurrent barb200_pecan_aligned_pairs_batch
+// callers, whose requests merge into one batch that the leader spreads over the devices.
+struct PecanState {
+    GroupCommit<PecanRequest> group;
+    std::vector<std::unique_ptr<PecanContext>> devs;
+};
+static PecanState &pecan_state(barb200_ctx *ctx) { return *(PecanState *)*pecan_slot(ctx); }
+static PecanContext &pecan_of(barb200_ctx *ctx, int dev) { return *pecan_state(ctx).devs[dev]; }
 
 namespace barb200 {
 int pecan_create(barb200_ctx *ctx) {
-    PecanContext *pc = new PecanContext();
-    *pecan_slot(ctx) = pc;
-    cudaFuncSetAttribute(pecan_posterior_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(pecan_posterior_kernel_r64, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    // wider classes hold longer jobs: they are launched first and at higher priority so that they are resident from the start
-    int prio_lo = 0, prio_hi = 0;
-    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    bool ok = cudaStreamCreateWithFlags(&pc->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaEventCreate(&pc->ev0) == cudaSuccess && cudaEventCreate(&pc->ev1) == cudaSuccess;
-    for (int c = 0; c < kNumClasses && ok; ++c)
-        ok = cudaStreamCreateWithPriority(&pc->cls[c], cudaStreamNonBlocking, kClass[c].threads <= 32 ? prio_lo : prio_hi) == cudaSuccess &&
-             cudaEventCreateWithFlags(&pc->done[c], cudaEventDisableTiming) == cudaSuccess;
+    PecanState *ps = new PecanState();
+    *pecan_slot(ctx) = ps;
+    bool ok = true;
+    for (int d = 0; d < ctx_device_count(ctx) && ok; ++d) {
+        PecanContext *pc = new PecanContext();
+        ps->devs.emplace_back(pc);
+        if (cudaSetDevice(ctx_device(ctx, d)) != cudaSuccess) { ok = false; break; }
+        cudaFuncSetAttribute(pecan_posterior_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        cudaFuncSetAttribute(pecan_posterior_kernel_r64, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        // wider classes hold longer jobs: they are launched first and at higher priority so that they are resident from the start
+        int prio_lo = 0, prio_hi = 0;
+        cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+        ok = cudaStreamCreateWithFlags(&pc->stream, cudaStreamNonBlocking) == cudaSuccess &&
+             cudaEventCreate(&pc->ev0) == cudaSuccess && cudaEventCreate(&pc->ev1) == cudaSuccess;
+        for (int c = 0; c < kNumClasses && ok; ++c)
+            ok = cudaStreamCreateWithPriority(&pc->cls[c], cudaStreamNonBlocking, kClass[c].threads <= 32 ? prio_lo : prio_hi) == cudaSuccess &&
+                 cudaEventCreateWithFlags(&pc->done[c], cudaEventDisableTiming) == cudaSuccess;
+    }
+    cudaSetDevice(ctx_device(ctx, 0));
     return ok ? 0 : -1;
 }
 
 void pecan_destroy(barb200_ctx *ctx) {
-    PecanContext *pc = (PecanContext *)*pecan_slot(ctx);
-    if (!pc) return;
-    if (pc->scratch) cudaFree(pc->scratch);
-    for (int c = 0; c < kNumClasses; ++c) { if (pc->cls[c]) cudaStreamDestroy(pc->cls[c]); if (pc->done[c]) cudaEventDestroy(pc->done[c]); }
-    if (pc->ev0) cudaEventDestroy(pc->ev0);
-    if (pc->ev1) cudaEventDestroy(pc->ev1);
-    if (pc->stream) cudaStreamDestroy(pc->stream);
-    delete pc;
+    PecanState *ps = (PecanState *)*pecan_slot(ctx);
+    if (!ps) return;
+    for (size_t d = 0; d < ps->devs.size(); ++d) {
+        PecanContext *pc = ps->devs[d].get();
+        cudaSetDevice(ctx_device(ctx, (int)d));
+        if (pc->scratch) cudaFree(pc->scratch);
+        for (int c = 0; c < kNumClasses; ++c) { if (pc->cls[c]) cudaStreamDestroy(pc->cls[c]); if (pc->done[c]) cudaEventDestroy(pc->done[c]); }
+        if (pc->ev0) cudaEventDestroy(pc->ev0);
+        if (pc->ev1) cudaEventDestroy(pc->ev1);
+        if (pc->stream) cudaStreamDestroy(pc->stream);
+    }
+    cudaSetDevice(ctx_device(ctx, 0));
+    delete ps;
 }
+
+void pecan_count_mum_pairs(barb200_ctx *ctx, int dev, int64_t n) { pecan_of(ctx, dev).mum_pairs += n; }
 }  // namespace barb200
 
 // a host staging buffer from the device's pinned pool, so that the copy runs at link speed; pageable memory if the pool cannot grow
 struct Staging {
-    barb200_ctx *ctx; void *pin = nullptr; size_t got = 0; std::vector<uint8_t> own;
-    explicit Staging(barb200_ctx *c) : ctx(c) {}
+    barb200_ctx *ctx; int dev; void *pin = nullptr; size_t got = 0; std::vector<uint8_t> own;
+    Staging(barb200_ctx *c, int d) : ctx(c), dev(d) {}
     ~Staging() { release(); }
     Staging(const Staging &) = delete; Staging &operator=(const Staging &) = delete;
     void *take(size_t bytes) {
-        pin = pinned_take(ctx, bytes, &got);
+        pin = pinned_take(ctx, dev, bytes, &got);
         if (pin) return pin;
         own.resize(bytes);
         return own.data();
     }
-    void release() { pinned_give(ctx, pin, got); pin = nullptr; std::vector<uint8_t>().swap(own); }
+    void release() { pinned_give(ctx, dev, pin, got); pin = nullptr; std::vector<uint8_t>().swap(own); }
 };
 
 struct PecanGroup {              // one launch: a class of jobs with one block shape
@@ -168,6 +197,7 @@ struct PecanGroup {              // one launch: a class of jobs with one block s
 
 struct barb200_pecan_stage {
     barb200_ctx *ctx = nullptr;
+    int dev = 0;                                 // the context's device the stage lives on (the staged C ABI: always 0)
     PlanParams P;
     Params devP;
     int64_t n_pairs = 0;
@@ -196,8 +226,8 @@ static unsigned pow2ceil(uint64_t v) { uint64_t p = 1024; while (p < v) p <<= 1;
 
 extern "C" void barb200_pecan_stage_destroy(barb200_pecan_stage *st) {
     if (!st) return;
-    cudaSetDevice(ctx_device(st->ctx));
-    for (auto &b : st->blocks) device_free(st->ctx, b.p, b.bytes);
+    cudaSetDevice(ctx_device(st->ctx, st->dev));
+    for (auto &b : st->blocks) device_free(st->ctx, st->dev, b.p, b.bytes);
     delete st;
 }
 
@@ -217,7 +247,8 @@ static int plan_params(barb200_ctx *ctx, const barb200_pecan_params *p, PlanPara
 // tables on the device, so it uploads only its job table and launch order.
 static int stage_build(barb200_pecan_stage *st, const char *const *sx, const char *const *sy, const barb200_pecan_stage *parent) {
     barb200_ctx *ctx = st->ctx;
-    PecanContext &pc = pecan_of(ctx);
+    const int dev = st->dev;
+    PecanContext &pc = pecan_of(ctx, dev);
     const int64_t ns = (int64_t)st->subs.size();
     std::string err;
     const int nthr = host_threads(ctx);
@@ -245,7 +276,7 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
     }
     st->cells = cells;
     // classes by the widest diagonal (kClass)
-    cudaSetDevice(ctx_device(ctx));
+    cudaSetDevice(ctx_device(ctx, dev));
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(ctx, cudaMemGetInfo(&free_b, &total_b));
     const size_t fixed = (size_t)sym_off + (size_t)band_off * 16 + (size_t)ns * (sizeof(Job) + 8) + (size_t)out_off * sizeof(Pair) * 2 + (64 << 20);
@@ -264,7 +295,7 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
         g.capM = pow2ceil((uint64_t)spanM); g.capF = pow2ceil((uint64_t)5 * (uint64_t)spanF);
         g.slot_doubles = (size_t)g.capM + g.capF + 11 * (size_t)(g.RW - g.RWs) + 8;
         g.smem_bytes = sizeof(double) * (K_TOTAL + 2 + 11 * (size_t)g.RWs);
-        g.ctas = (int)std::min<int64_t>((int64_t)ctx_sm_count(ctx) * kClass[c].ctas_per_sm, (int64_t)g.jobs.size());
+        g.ctas = (int)std::min<int64_t>((int64_t)ctx_sm_count(ctx, dev) * kClass[c].ctas_per_sm, (int64_t)g.jobs.size());
         std::sort(g.jobs.begin(), g.jobs.end(), [&](int a, int b) { return st->subs[a].cells != st->subs[b].cells ? st->subs[a].cells > st->subs[b].cells : a < b; });
         st->groups.push_back(std::move(g));
     }
@@ -292,7 +323,7 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
                     g.jobs.size(), kClass[g.cls].threads, g.ctas, g.RW, g.RWs, g.capM, g.capF, g.smem_bytes);
     // device arrays
     auto dev_alloc = [&](void **p, size_t bytes) -> bool {
-        if (device_alloc(ctx, p, bytes) != 0) return false;
+        if (device_alloc(ctx, dev, p, bytes) != 0) return false;
         st->blocks.push_back(barb200_pecan_stage::Block{*p, bytes});
         return true;
     };
@@ -305,7 +336,7 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
         set_error(ctx, "device allocation failed (pecan stage)"); return BARB200_ENOMEM;
     }
     if (!parent) st->d_sym = (uint8_t *)st->d_meta + meta_bytes;
-    Staging up(ctx);
+    Staging up(ctx, dev);
     Consts C; fill_constants(C);
     DiagMeta *meta = nullptr;                    // band tables, then symbols 0..4: the layout of d_meta / d_sym
     if (!parent) {
@@ -334,6 +365,12 @@ static int stage_build(barb200_pecan_stage *st, const char *const *sx, const cha
     return BARB200_OK;
 }
 
+// "" or why one input pair cannot be aligned
+static std::string pair_error(int64_t lx, int64_t ly, const int64_t *anchors, int64_t n_anchor) {
+    if (lx < 0 || ly < 0 || lx > 0x3fffffff || ly > 0x3fffffff || (n_anchor && !anchors)) return "bad sequence length or anchors";
+    return check_anchors(anchors, n_anchor, lx, ly);
+}
+
 static int stage_create_impl(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                              const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                              const int64_t *const *anchors, const int64_t *n_anchor,
@@ -348,8 +385,7 @@ static int stage_create_impl(barb200_ctx *ctx, const barb200_pecan_params *p, in
     for (int64_t i = 0; i < n_pairs; ++i) {
         const int64_t na = n_anchor ? n_anchor[i] : 0;
         const int64_t *a = (anchors && na) ? anchors[i] : nullptr;
-        if (lx[i] < 0 || ly[i] < 0 || lx[i] > 0x3fffffff || ly[i] > 0x3fffffff || (na && !a)) { set_error(ctx, "bad sequence length or anchors"); delete st; return BARB200_EINVAL; }
-        const std::string e = check_anchors(a, na, lx[i], ly[i]);
+        const std::string e = pair_error(lx[i], ly[i], a, na);
         if (!e.empty()) { set_error(ctx, e); delete st; return BARB200_EINVAL; }
         st->pair_first[i] = (int64_t)st->subs.size();
         split_pair(P, i, lx[i], ly[i], a, na, ragged_left && ragged_left[i], ragged_right && ragged_right[i], st->subs);
@@ -366,14 +402,14 @@ extern "C" int barb200_pecan_stage_create(barb200_ctx *ctx, const barb200_pecan_
                                           const int64_t *const *anchors, const int64_t *n_anchor,
                                           const uint8_t *ragged_left, const uint8_t *ragged_right, barb200_pecan_stage **out) {
     if (!ctx) return BARB200_EINVAL;
-    std::lock_guard<std::mutex> lk(pecan_of(ctx).mu);
+    std::lock_guard<std::mutex> lk(pecan_of(ctx, 0).mu);
     return stage_create_impl(ctx, p, n_pairs, sx, lx, sy, ly, anchors, n_anchor, ragged_left, ragged_right, out);
 }
 
 static int stage_run_locked(barb200_pecan_stage *st, float *kernel_ms) {
     barb200_ctx *ctx = st->ctx;
-    PecanContext &pc = pecan_of(ctx);
-    cudaSetDevice(ctx_device(ctx));
+    PecanContext &pc = pecan_of(ctx, st->dev);
+    cudaSetDevice(ctx_device(ctx, st->dev));
     if (pc.scratch_bytes < st->scratch_bytes) {      // grow the context's rings
         cudaFree(pc.scratch);
         pc.scratch_bytes = 0;
@@ -412,7 +448,7 @@ static int stage_run_locked(barb200_pecan_stage *st, float *kernel_ms) {
 
 extern "C" int barb200_pecan_stage_run(barb200_pecan_stage *st, float *kernel_ms) {
     if (!st) return BARB200_EINVAL;
-    std::lock_guard<std::mutex> lk(pecan_of(st->ctx).mu);
+    std::lock_guard<std::mutex> lk(pecan_of(st->ctx, st->dev).mu);
     return stage_run_locked(st, kernel_ms);
 }
 
@@ -422,10 +458,11 @@ extern "C" int64_t barb200_pecan_stage_launches(barb200_pecan_stage *st) { retur
 // candidates of every sub-job, in emission order (host copies); overflowed jobs are re-run with room for every cell
 static int stage_collect(barb200_pecan_stage *st, std::vector<std::vector<Pair>> &per_sub) {
     barb200_ctx *ctx = st->ctx;
+    const int dev = st->dev;
     const int64_t ns = (int64_t)st->subs.size();
     per_sub.assign(ns, std::vector<Pair>());
     if (ns == 0) return BARB200_OK;
-    cudaSetDevice(ctx_device(ctx));
+    cudaSetDevice(ctx_device(ctx, dev));
     std::vector<int> out_n(ns);
     CUDA_TRY(ctx, cudaMemcpy(out_n.data(), st->d_out_n, sizeof(int) * ns, cudaMemcpyDeviceToHost));
     std::vector<long long> dst_off(ns + 1, 0);
@@ -436,22 +473,22 @@ static int stage_collect(barb200_pecan_stage *st, std::vector<std::vector<Pair>>
         dst_off[i + 1] = dst_off[i] + (over ? 0 : out_n[i]);
     }
     const long long total = dst_off[ns];
-    Staging down(ctx);
+    Staging down(ctx, dev);
     Pair *const flat = total > 0 ? (Pair *)down.take(sizeof(Pair) * (size_t)total) : nullptr;
     if (total > 0) {
         long long *d_dst_off = nullptr; Pair *d_flat = nullptr;
-        if (device_alloc(ctx, (void **)&d_dst_off, sizeof(long long) * (ns + 1)) != 0) { set_error(ctx, "device allocation failed (compact offsets)"); return BARB200_ENOMEM; }
+        if (device_alloc(ctx, dev, (void **)&d_dst_off, sizeof(long long) * (ns + 1)) != 0) { set_error(ctx, "device allocation failed (compact offsets)"); return BARB200_ENOMEM; }
         cudaError_t e = cudaSuccess;
-        if (device_alloc(ctx, (void **)&d_flat, sizeof(Pair) * (size_t)total) != 0) {
-            device_free(ctx, d_dst_off, sizeof(long long) * (ns + 1)); set_error(ctx, "device allocation failed (compact output)"); return BARB200_ENOMEM; }
-        cudaStream_t s = pecan_of(ctx).stream;
+        if (device_alloc(ctx, dev, (void **)&d_flat, sizeof(Pair) * (size_t)total) != 0) {
+            device_free(ctx, dev, d_dst_off, sizeof(long long) * (ns + 1)); set_error(ctx, "device allocation failed (compact output)"); return BARB200_ENOMEM; }
+        cudaStream_t s = pecan_of(ctx, dev).stream;
         cudaMemcpyAsync(d_dst_off, dst_off.data(), sizeof(long long) * (ns + 1), cudaMemcpyHostToDevice, s);
-        const int grid = (int)std::min<int64_t>(ns, (int64_t)ctx_sm_count(ctx) * 16);
+        const int grid = (int)std::min<int64_t>(ns, (int64_t)ctx_sm_count(ctx, dev) * 16);
         pecan_compact_kernel<<<grid, 128, 0, s>>>(st->d_jobs, st->d_out_n, d_dst_off, st->d_out, d_flat, (int)ns);
         ++st->launches;
         cudaMemcpyAsync(flat, d_flat, sizeof(Pair) * (size_t)total, cudaMemcpyDeviceToHost, s);
         e = cudaStreamSynchronize(s);
-        device_free(ctx, d_dst_off, sizeof(long long) * (ns + 1)); device_free(ctx, d_flat, sizeof(Pair) * (size_t)total);
+        device_free(ctx, dev, d_dst_off, sizeof(long long) * (ns + 1)); device_free(ctx, dev, d_flat, sizeof(Pair) * (size_t)total);
         if (e != cudaSuccess) { set_error(ctx, std::string("pecan compaction: ") + cudaGetErrorString(e)); return BARB200_ECUDA; }
     }
     const int nthr = host_threads(ctx);
@@ -480,8 +517,8 @@ static int stage_collect(barb200_pecan_stage *st, std::vector<std::vector<Pair>>
     down.release();
     if (!retry.empty()) {
         if (st->full_cap) { set_error(ctx, "pecan: output overflow with full capacity (internal error)"); return BARB200_EJOB; }
-        barb200_pecan_stage *rs = new barb200_pecan_stage();
-        rs->ctx = ctx; rs->P = st->P; rs->full_cap = true;
+        barb200_pecan_stage *rs = new barb200_pecan_stage();   // on the parent's device: it reads the parent's symbols and bands
+        rs->ctx = ctx; rs->dev = dev; rs->P = st->P; rs->full_cap = true;
         for (int64_t i : retry) { rs->subs.push_back(st->subs[i]); rs->jobs.push_back(st->jobs[i]); }
         int rc = stage_build(rs, nullptr, nullptr, st);
         if (rc == BARB200_OK) rc = stage_run_locked(rs, nullptr);
@@ -539,28 +576,30 @@ extern "C" int barb200_pecan_stage_fetch(barb200_pecan_stage *st, int64_t **trip
     std::vector<std::vector<Pair>> per_sub;
     int rc;
     {
-        std::lock_guard<std::mutex> lk(pecan_of(st->ctx).mu);
+        std::lock_guard<std::mutex> lk(pecan_of(st->ctx, st->dev).mu);
         rc = stage_collect(st, per_sub);
     }
     if (rc) return rc;
     return finish_pairs(st, per_sub, triples_out, n_out, posteriors_out, cells_out);
 }
 
+// chunks bounded by the output room a stage reserves (16 B per candidate, ~ (lx + ly) candidates per pair)
+static const int64_t kChunkRecords = (int64_t)128 << 20;
+
+// The batch on a single-device context: chunks of pairs in caller order, each split, planned, run and finished as one stage.
 static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                            const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                            const int64_t *const *anchors, const int64_t *n_anchor,
                            const uint8_t *ragged_left, const uint8_t *ragged_right,
                            int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out) {
     if (!ctx || !triples_out || !n_out) { if (ctx) set_error(ctx, "bad argument"); return BARB200_EINVAL; }
-    // chunks bounded by the output room a stage reserves (16 B per candidate, ~ (lx + ly) candidates per pair)
-    const int64_t kChunkRecords = (int64_t)128 << 20;
     int64_t i0 = 0;
     while (i0 < n_pairs || (n_pairs == 0 && i0 == 0)) {
         int64_t i1 = i0, rec = 0;
         while (i1 < n_pairs && (i1 == i0 || rec + lx[i1] + ly[i1] + 64 <= kChunkRecords)) { rec += lx[i1] + ly[i1] + 64; ++i1; }
         barb200_pecan_stage *st = nullptr;
         const double t0 = omp_get_wtime();
-        std::unique_lock<std::mutex> lk(pecan_of(ctx).mu);      // held from create to collect, like a stage's three calls
+        std::unique_lock<std::mutex> lk(pecan_of(ctx, 0).mu);   // held from create to collect, like a stage's three calls
         int rc = stage_create_impl(ctx, p, i1 - i0, sx + i0, lx + i0, sy + i0, ly + i0, anchors ? anchors + i0 : nullptr,
                                    n_anchor ? n_anchor + i0 : nullptr, ragged_left ? ragged_left + i0 : nullptr,
                                    ragged_right ? ragged_right + i0 : nullptr, &st);
@@ -577,14 +616,116 @@ static int pecan_batch_now(barb200_ctx *ctx, const barb200_pecan_params *p, int6
         if (getenv("BARB200_DEBUG")) fprintf(stderr, "[barb200] pecan batch of %lld pairs: create %.1f ms, run %.1f ms, fetch %.1f ms, destroy %.1f ms\n",
                                              (long long)(i1 - i0), (t1 - t0) * 1e3, (t2 - t1) * 1e3, (t3 - t2) * 1e3, (omp_get_wtime() - t3) * 1e3);
         if (rc) return rc;
+        pecan_of(ctx, 0).hmm_pairs += i1 - i0;
         if (n_pairs == 0) break;
         i0 = i1;
     }
     return BARB200_OK;
 }
 
+// One chunk of device `dev`'s share: the caller's pairs pairs[0, n), already split and planned (subs[caller index], moved into the
+// stage), run on the device and finished; the outputs land at the caller's indices, also when a step fails (the caller frees them).
+static int pecan_chunk_on_device(barb200_ctx *ctx, int dev, const PlanParams &P, const int64_t *pairs, int64_t n, std::vector<std::vector<SubJob>> &subs,
+                                 const char *const *sx, const char *const *sy, int64_t **triples_out, int64_t *n_out, double **posteriors_out,
+                                 int64_t *cells_out) {
+    barb200_pecan_stage *st = new barb200_pecan_stage();
+    st->ctx = ctx; st->dev = dev; st->P = P; st->n_pairs = n;
+    st->pair_first.assign(n + 1, 0);
+    std::vector<const char *> csx(n), csy(n);
+    for (int64_t k = 0; k < n; ++k) {
+        csx[k] = sx[pairs[k]]; csy[k] = sy[pairs[k]];
+        st->pair_first[k] = (int64_t)st->subs.size();
+        for (SubJob &s : subs[pairs[k]]) { s.pair = k; st->subs.push_back(std::move(s)); }
+    }
+    st->pair_first[n] = (int64_t)st->subs.size();
+    std::vector<int64_t *> trip(n, nullptr); std::vector<double *> post(n, nullptr); std::vector<int64_t> no(n, 0), cells(n, 0);
+    std::vector<std::vector<Pair>> per_sub;
+    int rc;
+    {
+        std::lock_guard<std::mutex> lk(pecan_of(ctx, dev).mu);
+        rc = stage_build(st, csx.data(), csy.data(), nullptr);
+        if (rc == BARB200_OK) rc = stage_run_locked(st, nullptr);
+        if (rc == BARB200_OK) rc = stage_collect(st, per_sub);
+    }
+    if (rc == BARB200_OK) rc = finish_pairs(st, per_sub, trip.data(), no.data(), posteriors_out ? post.data() : nullptr, cells.data());
+    barb200_pecan_stage_destroy(st);
+    for (int64_t k = 0; k < n; ++k) {
+        const int64_t i = pairs[k];
+        triples_out[i] = trip[k]; n_out[i] = no[k];
+        if (posteriors_out) posteriors_out[i] = post[k];
+        if (cells_out) cells_out[i] = cells[k];
+    }
+    if (rc == BARB200_OK) pecan_of(ctx, dev).hmm_pairs += n;
+    return rc;
+}
+
+// The batch on a context of several devices. Every pair is checked, split and planned once here; the pairs are dealt to the
+// devices by their planned cells (deal_pairs), and each device runs its share in chunks (as pecan_batch_now) on a host thread
+// of its own. Results are the single-device results, bit for bit: a job's posteriors do not depend on the jobs beside it.
+// If a device fails, the whole request fails with that device's message and no outputs.
+static int pecan_batch_devices(barb200_ctx *ctx, int ndev, const barb200_pecan_params *p, int64_t n_pairs,
+                               const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
+                               const int64_t *const *anchors, const int64_t *n_anchor,
+                               const uint8_t *ragged_left, const uint8_t *ragged_right,
+                               int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out) {
+    PlanParams P;
+    int rc = plan_params(ctx, p, P);
+    if (rc) return rc;
+    std::vector<std::vector<SubJob>> subs(n_pairs);
+    std::vector<int64_t> cost(n_pairs, 0);
+    std::string err; int64_t err_at = n_pairs;
+#pragma omp parallel for schedule(dynamic, 16) num_threads(host_threads(ctx))
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int64_t na = n_anchor ? n_anchor[i] : 0;
+        const int64_t *a = (anchors && na) ? anchors[i] : nullptr;
+        std::string e = pair_error(lx[i], ly[i], a, na);
+        if (e.empty()) {
+            split_pair(P, i, lx[i], ly[i], a, na, ragged_left && ragged_left[i], ragged_right && ragged_right[i], subs[i]);
+            for (SubJob &s : subs[i]) { if (!(e = plan_subjob(P, s)).empty()) break; cost[i] += s.cells; }
+        }
+        if (!e.empty()) {
+#pragma omp critical
+            if (i < err_at) { err_at = i; err = e; }       // the first bad pair's message, whichever thread finds it
+        }
+    }
+    if (!err.empty()) { set_error(ctx, err); return BARB200_EINVAL; }
+    for (int64_t i = 0; i < n_pairs; ++i) { triples_out[i] = nullptr; n_out[i] = 0; if (posteriors_out) posteriors_out[i] = nullptr; }
+    const std::vector<std::vector<int64_t>> share = deal_pairs(cost, ndev);
+    int active = 0;
+    for (const auto &s : share) active += !s.empty();
+    std::vector<int> rcs(ndev, BARB200_OK);
+    std::vector<std::string> errs(ndev);
+    auto run_device = [&](int d) {
+        set_host_thread_share(active);
+        const std::vector<int64_t> &mine = share[d];
+        try {
+            for (size_t at = 0; at < mine.size();) {
+                size_t end = at; int64_t rec = 0;
+                while (end < mine.size() && (end == at || rec + lx[mine[end]] + ly[mine[end]] + 64 <= kChunkRecords)) { rec += lx[mine[end]] + ly[mine[end]] + 64; ++end; }
+                const int r = pecan_chunk_on_device(ctx, d, P, mine.data() + at, (int64_t)(end - at), subs, sx, sy, triples_out, n_out, posteriors_out, cells_out);
+                if (r) { rcs[d] = r; errs[d] = get_error(ctx); break; }
+                at = end;
+            }
+        } catch (const std::bad_alloc &) { rcs[d] = BARB200_ENOMEM; errs[d] = "host allocation failed"; }
+        set_host_thread_share(1);
+    };
+    std::vector<std::thread> th;
+    for (int d = 0; d < ndev; ++d) if (!share[d].empty()) th.emplace_back(run_device, d);
+    for (auto &t : th) t.join();
+    for (int d = 0; d < ndev; ++d) if (rcs[d]) {
+        for (int64_t i = 0; i < n_pairs; ++i) {
+            free(triples_out[i]); triples_out[i] = nullptr; n_out[i] = 0;
+            if (posteriors_out) { free(posteriors_out[i]); posteriors_out[i] = nullptr; }
+        }
+        set_error(ctx, errs[d]);
+        return rcs[d];
+    }
+    return BARB200_OK;
+}
+
 // Concurrent callers (one per OpenMP thread of bar(), bar/impl/bar.c:90-94) share device batches: whatever is waiting when the
-// device becomes free runs as ONE batch (group_commit.h, batch_merge.h); a single caller runs its own request unchanged.
+// device becomes free runs as ONE batch (group_commit.h, batch_merge.h); a single caller runs its own request unchanged. On a
+// context of several devices the leader spreads that batch over them (pecan_batch_devices).
 extern "C" int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                                                  const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                                                  const int64_t *const *anchors, const int64_t *n_anchor,
@@ -595,14 +736,27 @@ extern "C" int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200
     r.p = *p; r.n = n_pairs; r.sx = sx; r.lx = lx; r.sy = sy; r.ly = ly; r.anchors = anchors; r.n_anchor = n_anchor;
     r.ragged_left = ragged_left; r.ragged_right = ragged_right;
     r.triples_out = triples_out; r.n_out = n_out; r.posteriors_out = posteriors_out; r.cells_out = cells_out;
-    pecan_of(ctx).group.submit(&r, pecan_can_merge, [ctx](std::vector<PecanRequest *> &batch) {
-        run_pecan_group(batch, [ctx](const barb200_pecan_params *pp, int64_t n, const char *const *a, const int64_t *la, const char *const *b, const int64_t *lb,
-                                     const int64_t *const *an, const int64_t *na, const uint8_t *rl, const uint8_t *rr, int64_t **trip, int64_t *no,
-                                     double **post, int64_t *cells) {
-            return pecan_batch_now(ctx, pp, n, a, la, b, lb, an, na, rl, rr, trip, no, post, cells);
+    const int ndev = ctx_device_count(ctx);
+    pecan_state(ctx).group.submit(&r, pecan_can_merge, [ctx, ndev](std::vector<PecanRequest *> &batch) {
+        run_pecan_group(batch, [ctx, ndev](const barb200_pecan_params *pp, int64_t n, const char *const *a, const int64_t *la, const char *const *b, const int64_t *lb,
+                                           const int64_t *const *an, const int64_t *na, const uint8_t *rl, const uint8_t *rr, int64_t **trip, int64_t *no,
+                                           double **post, int64_t *cells) {
+            return ndev == 1 ? pecan_batch_now(ctx, pp, n, a, la, b, lb, an, na, rl, rr, trip, no, post, cells)
+                             : pecan_batch_devices(ctx, ndev, pp, n, a, la, b, lb, an, na, rl, rr, trip, no, post, cells);
         });
     });
     return r.rc;
+}
+
+extern "C" int barb200_pecan_device_stats(barb200_ctx *ctx, int64_t *hmm_pairs, int64_t *mum_pairs, int max_devices) {
+    if (!ctx) return BARB200_EINVAL;
+    const PecanState &ps = pecan_state(ctx);
+    const int n = (int)ps.devs.size();
+    for (int d = 0; d < n && d < max_devices; ++d) {
+        if (hmm_pairs) hmm_pairs[d] = ps.devs[d]->hmm_pairs.load();
+        if (mum_pairs) mum_pairs[d] = ps.devs[d]->mum_pairs.load();
+    }
+    return n;
 }
 
 extern "C" int barb200_pecan_band(int64_t lx, int64_t ly, const int64_t *anchors, int64_t n_anchor, int64_t expansion, int64_t *xmy_l, int64_t *xmy_r) {

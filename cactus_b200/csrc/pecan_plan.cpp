@@ -148,5 +148,19 @@ std::string plan_subjob(const PlanParams &P, SubJob &s) {
     return "";
 }
 
+std::vector<std::vector<int64_t>> deal_pairs(const std::vector<int64_t> &cost, int ndev) {
+    const int64_t n = (int64_t)cost.size();
+    ndev = std::max(ndev, 1);
+    std::vector<std::vector<int64_t>> share(ndev);
+    std::vector<int64_t> idx(n);
+    for (int64_t i = 0; i < n; ++i) idx[i] = i;
+    if (ndev == 1) { share[0] = std::move(idx); return share; }
+    std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return cost[a] > cost[b]; });
+    std::vector<int64_t> load(ndev, 0);
+    for (int64_t i : idx) { const int d = (int)(std::min_element(load.begin(), load.end()) - load.begin()); share[d].push_back(i); load[d] += cost[i]; }
+    for (auto &s : share) std::sort(s.begin(), s.end());
+    return share;
+}
+
 }  // namespace pecan
 }  // namespace barb200

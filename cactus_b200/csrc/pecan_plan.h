@@ -50,6 +50,11 @@ void split_pair(const PlanParams &P, int64_t pair, int64_t lx, int64_t ly, const
 // the two diagonals the forward sweep resumes from after an intermediate traceback. Returns "" or an error.
 std::string plan_subjob(const PlanParams &P, SubJob &j);
 
+// A batch over ndev devices: whole pairs by cost (a pair-HMM pair: the planned cells of its sub-jobs; a MUM-anchor pair: its
+// device bytes), largest first to the least-loaded device (ties: the lower device; equal costs: the earlier pair), every share
+// in caller order. One device takes every pair in caller order. Returns ndev shares of indices into `cost`.
+std::vector<std::vector<int64_t>> deal_pairs(const std::vector<int64_t> &cost, int ndev);
+
 // The reference's order of emission inside one sub-matrix (getPosteriorProbsWithBanding): tracebacks in increasing order of
 // their start diagonal, inside a traceback diagonals x+y downwards, inside a diagonal x - y (hence x) upwards.
 // Sort key of the candidate (0-based x, y) of sub-job j; ascending (first, second) = order of emission.

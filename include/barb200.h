@@ -159,7 +159,10 @@ void barb200_pecan_params_default(barb200_pecan_params *p);
  * int64 (score = floor(posterior * PAIR_ALIGNMENT_PROB_1), x, y) in the order the reference returns them;
  * posteriors_out (may be NULL) receives malloc'd doubles, the pre-floor posteriors exp(f_M + b_M - total);
  * cells_out (may be NULL) the banded DP cells of the pair (sum of diagonal widths over its sub-matrices).
- * Release every array with barb200_free. */
+ * Release every array with barb200_free.
+ * Several devices (barb200_params.n_devices): whole pairs are dealt to the context's devices by their banded cells and every
+ * device runs its share at once; the outputs are those of a single-device context, bit for bit. If any device fails, the call
+ * fails with that device's message and leaves no outputs. */
 int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                                       const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                                       const int64_t *const *anchors, const int64_t *n_anchor,
@@ -167,7 +170,8 @@ int barb200_pecan_aligned_pairs_batch(barb200_ctx *ctx, const barb200_pecan_para
                                       int64_t **triples_out, int64_t *n_out, double **posteriors_out, int64_t *cells_out);
 
 /* Staged form (inputs resident in HBM; used by bench.py): create = split + band + pack + H2D; run = kernels only
- * (repeatable); fetch = compaction + D2H + exp/threshold/floor on the host. */
+ * (repeatable); fetch = compaction + D2H + exp/threshold/floor on the host. A stage lives on the context's first device,
+ * whatever the number of devices. */
 typedef struct barb200_pecan_stage barb200_pecan_stage;
 int barb200_pecan_stage_create(barb200_ctx *ctx, const barb200_pecan_params *p, int64_t n_pairs,
                                const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
@@ -205,13 +209,22 @@ void barb200_mum_params_default(barb200_mum_params *p);
 /* For pair i: NUL-free 7-bit ASCII strings sx[i] (length lx[i]) and sy[i] (ly[i]). anchors_out[i] = malloc'd n_anchor_out[i] x 2
  * int64 (x, y), 0-based, in the reference's order -- strictly increasing in both with recursive_mums (what
  * barb200_pecan_aligned_pairs_batch takes), last MUM first and each MUM backwards without. Release with barb200_free.
- * BARB200_EINVAL for k outside 1..64, u < 0, or a NUL / non-ASCII byte. */
+ * BARB200_EINVAL for k outside 1..64, u < 0, or a NUL / non-ASCII byte.
+ * Several devices: the pairs larger than anchor_matrix_bigger_than_this are dealt to the context's devices by the device memory
+ * they take, and every device runs its share at once; the anchors are those of a single-device context. */
 int barb200_pecan_anchor_pairs_batch(barb200_ctx *ctx, const barb200_mum_params *p, int64_t n_pairs,
                                      const char *const *sx, const int64_t *lx, const char *const *sy, const int64_t *ly,
                                      int64_t **anchors_out, int64_t *n_anchor_out);
-/* The calling thread's last barb200_pecan_anchor_pairs_batch: out[0] device time of its kernels and copies (ms), out[1] wall
- * time of the call (ms), out[2] kernels launched. For reports. */
+/* The calling thread's last barb200_pecan_anchor_pairs_batch: out[0] device time of its kernels and copies (ms; with several
+ * devices, that of the device that took longest), out[1] wall time of the call (ms), out[2] kernels launched on all devices.
+ * For reports. */
 int barb200_mum_last_timing(double out[3]);
+
+/* Per device of the context (up to max_devices entries; either array may be NULL): the sequence pairs
+ * barb200_pecan_aligned_pairs_batch (hmm_pairs) and barb200_pecan_anchor_pairs_batch (mum_pairs, only pairs that needed the
+ * device) have run there since the context was created; the staged form is not counted. Returns the number of devices of the
+ * context. For reports and tests. */
+int barb200_pecan_device_stats(barb200_ctx *ctx, int64_t *hmm_pairs, int64_t *mum_pairs, int max_devices);
 
 /* ------------------------------------------------------------------------------------------------------------
  * The end queue, asynchronously. barb200_flower_submit takes the arguments of make_consistent_partial_order_alignments

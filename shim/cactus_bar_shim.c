@@ -23,6 +23,7 @@
 #include <string.h>
 #include "poaBarAligner.h"
 #include "barb200.h"
+#include "barb200_shim_env.h"
 
 static pthread_mutex_t shim_mutex = PTHREAD_MUTEX_INITIALIZER;
 /* one engine per distinct parameter set, created on first use and kept for the life of the process: another OpenMP thread
@@ -41,21 +42,7 @@ static void params_from_abpoa(const abpoa_para_t *abpt, barb200_params *p) {
     p->k = abpt->k; p->w = abpt->w; p->min_w = abpt->min_w;
     p->progressive_poa = abpt->progressive_poa;
     p->disable_seeding = abpt->disable_seeding;
-    const char *dev = getenv("BARB200_DEVICE");          /* one GPU for this process ... */
-    if (dev) p->device = atoi(dev);
-    const char *devs = getenv("BARB200_DEVICES");        /* ... or several behind ONE context: "all" or "0,1,2,3" */
-    if (devs) {
-        if (strcmp(devs, "all") == 0) {
-            p->n_devices = -1;
-        } else {
-            p->n_devices = 0;
-            for (const char *c = devs; *c && p->n_devices < 8; ) {
-                p->devices[p->n_devices++] = atoi(c);
-                while (*c && *c != ',') c++;
-                if (*c == ',') c++;
-            }
-        }
-    }
+    barb200_devices_from_env(p);                          /* BARB200_DEVICE / BARB200_DEVICES */
 }
 
 /* field-wise comparison (memcmp would read struct padding) */

@@ -30,6 +30,7 @@
 #include "multipleAligner.h"
 #include "stateMachine.h"
 #include "barb200.h"
+#include "barb200_shim_env.h"
 
 /* defined in impl/pairwiseAligner.c:1222-1233 (not static) but missing from pairwiseAligner.h */
 stList *getAnchorPairsForPairwiseAlignmentParameters(const char *sX, const char *sY, const int64_t lX, const int64_t lY,
@@ -44,8 +45,7 @@ static barb200_ctx *shim_context(void) {
         barb200_params p;
         char err[256];
         barb200_params_default(&p);                       /* the POA fields are not used by the pair-HMM path */
-        const char *dev = getenv("BARB200_DEVICE");
-        if (dev) p.device = atoi(dev);
+        barb200_devices_from_env(&p);                     /* BARB200_DEVICE / BARB200_DEVICES, as in POA mode */
         shim_ctx = barb200_create(&p, err, (int)sizeof(err));
         if (shim_ctx == NULL) {
             pthread_mutex_unlock(&shim_mutex);
