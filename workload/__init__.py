@@ -34,6 +34,8 @@ def _lib():
         lib.barsynth_pair.restype = i64
         lib.barsynth_msa_hash.argtypes = [vp, i64, ci]
         lib.barsynth_msa_hash.restype = C.c_uint64
+        lib.barsynth_fnv1a.argtypes = [vp, i64]
+        lib.barsynth_fnv1a.restype = C.c_uint64
         _LIB = lib
     return _LIB
 
@@ -146,3 +148,54 @@ def read_harvest(path):
         out.append({"ends": ends, "right_end_indexes": None if single else ri, "right_end_row_indexes": None if single else rr,
                     "overlaps": None if single else ov, "window_size": window, "max_prog_rows": max_rows, "max_prog_length_diff": diff})
     return out
+
+
+PECAN_HARVEST_MAGIC = 0x484E435032303042
+PECAN_PARAM_FIELDS = ("min_diags_between_traceback", "traceback_diagonals", "diagonal_expansion", "split_matrix_bigger_than_this",
+                      "dynamic_anchor_expansion")
+MUM_PARAM_FIELDS = ("anchor_matrix_bigger_than_this", "k", "u", "recursive_mums")
+
+
+def read_pecan_harvest(path):
+    """Sequence pairs recorded by shim/cactus_pecan_harvest.c (BARB200_PECAN_HARVEST=<path>) during a reference cPecan-mode bar()
+    run -> list of ends in the order their first pair was recorded, each {"end": end id, "pairs": [pair, ...]} with the pairs
+    in recorded order. A pair is a dict: "end", "index" (its number within the end), "sx", "sy" (bytes), "ragged_left",
+    "ragged_right", "use_mum_anchors" (bool), "pecan" (threshold and the barb200_pecan_params fields), "mum" (the
+    barb200_mum_params fields), "anchors" (int64 [n, 2], the reference's), "anchor_hash", "n_triples", "triple_hash".
+    Raises ValueError naming the byte offset of a record with a bad magic or one cut short."""
+    import struct
+    with open(path, "rb") as f:
+        data = f.read()
+    head = struct.Struct("<qqqd" + "q" * 15 + "QqQ")
+    ends, order, o = {}, [], 0
+    while o < len(data):
+        start = o
+        if len(data) - o >= 8 and struct.unpack_from("<q", data, o)[0] != PECAN_HARVEST_MAGIC:
+            raise ValueError("bad pecan harvest record at byte %d: no magic number" % start)
+        if len(data) - o < head.size:
+            raise ValueError("pecan harvest record at byte %d is truncated" % start)
+        v = head.unpack_from(data, o)
+        o += head.size
+        (_, end, index, threshold), ints, (anchor_hash, n_triples, triple_hash) = v[:4], v[4:19], v[19:]
+        lx, ly, na = ints[12:15]
+        if min(lx, ly, na) < 0 or len(data) - o < lx + ly + 16 * na:
+            raise ValueError("pecan harvest record at byte %d is truncated" % start)
+        sx, sy = data[o:o + lx], data[o + lx:o + lx + ly]
+        o += lx + ly
+        anchors = np.frombuffer(data, np.int64, 2 * na, o).reshape(na, 2).copy()
+        o += 16 * na
+        pair = {"end": end, "index": index, "sx": sx, "sy": sy, "ragged_left": bool(ints[10]), "ragged_right": bool(ints[11]),
+                "use_mum_anchors": bool(ints[9]), "pecan": dict(zip(PECAN_PARAM_FIELDS, ints[0:5]), threshold=threshold),
+                "mum": dict(zip(MUM_PARAM_FIELDS, ints[5:9])),
+                "anchors": anchors, "anchor_hash": anchor_hash, "n_triples": n_triples, "triple_hash": triple_hash}
+        if end not in ends:
+            ends[end] = {"end": end, "pairs": []}
+            order.append(end)
+        ends[end]["pairs"].append(pair)
+    return [ends[e] for e in order]
+
+
+def fnv1a64(words):
+    """64-bit FNV-1a over the little-endian bytes of an int64 array: the anchor and triple hashes of a pecan harvest record"""
+    w = np.ascontiguousarray(words, "<i8")
+    return int(_lib().barsynth_fnv1a(w.ctypes.data, w.nbytes))

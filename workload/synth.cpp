@@ -108,3 +108,10 @@ extern "C" uint64_t barsynth_msa_hash(const uint8_t *m, int64_t n, int msa_len) 
     for (int64_t k = 0; k < n; ++k) { h ^= m[k]; h *= 1099511628211ULL; }
     return h;
 }
+
+// plain 64-bit FNV-1a over n bytes: the anchor and triple hashes of a cPecan harvest record (shim/cactus_pecan_harvest.c)
+extern "C" uint64_t barsynth_fnv1a(const uint8_t *b, int64_t n) {
+    uint64_t h = 0xcbf29ce484222325ULL;
+    for (int64_t k = 0; k < n; ++k) { h ^= b[k]; h *= 0x100000001b3ULL; }
+    return h;
+}
