@@ -74,6 +74,8 @@ def load_library():
     lib.barb200_last_error.restype = C.c_char_p
     lib.barb200_poa_msa_batch.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp, vp]
     lib.barb200_poa_msa_batch.restype = ci
+    lib.barb200_poa_trace_batch.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp]
+    lib.barb200_poa_trace_batch.restype = ci
     lib.barb200_stage_create.argtypes = [vp, i64, vp, vp, vp, vp, C.POINTER(vp)]
     lib.barb200_stage_create.restype = ci
     lib.barb200_stage_run.argtypes = [vp, C.POINTER(C.c_float)]
@@ -159,6 +161,56 @@ def msa_to_base(n):
 def msa_to_byte(c):
     """bar/impl/poaBarAligner.c:159-161"""
     return {"A": 0, "a": 0, "C": 1, "c": 1, "G": 2, "g": 2, "T": 3, "t": 3, "-": 5}.get(c, 4)
+
+
+def parse_trace(words, n_seq):
+    """One job's trace words (barb200_poa_trace_batch, layout in include/barb200.h) as a dict: msa (uint8 [n_seq, msa_len]), msa_len,
+    cells, read_id_map, alns = one dict per alignment in read order with read_id, qlen, node_n, best_score, cigar (uint64),
+    dp_beg and dp_end (int32 per row). abPOA's per-alignment state has the same layout, so a reference dump parses alike."""
+    w = np.asarray(words, np.int64)
+    if int(w[0]) != n_seq:
+        raise ValueError("trace of %d sequences, expected %d" % (int(w[0]), n_seq))
+    msa_len, cells = int(w[1]), int(w[2])
+    pos = 3
+    read_id_map = [int(x) for x in w[pos:pos + n_seq]]
+    pos += n_seq
+    alns = []
+    for _ in range(n_seq):
+        read_id, qlen, node_n, n_cigar, best, n_rows = (int(x) for x in w[pos:pos + 6])
+        pos += 6
+        cigar = w[pos:pos + n_cigar].astype(np.uint64, copy=True)
+        pos += n_cigar
+        dp_beg = w[pos:pos + n_rows].astype(np.int32)
+        pos += n_rows
+        dp_end = w[pos:pos + n_rows].astype(np.int32)
+        pos += n_rows
+        alns.append(dict(read_id=read_id, qlen=qlen, node_n=node_n, best_score=best, cigar=cigar, dp_beg=dp_beg, dp_end=dp_end))
+    msa = w[pos:].view(np.uint8)[: n_seq * msa_len].reshape(n_seq, msa_len).copy()
+    return dict(msa=msa, msa_len=msa_len, cells=cells, read_id_map=read_id_map, alns=alns)
+
+
+def first_trace_difference(got, want):
+    """Where two traces of one job (dicts of :func:`parse_trace`) first differ: None, or (alignment, field, index). alignment is None
+    for the job's own fields (read order, MSA length, cells, MSA); index is the first differing entry of a cigar or band array, a
+    "length a vs b" note when their lengths differ, and None for scalar fields."""
+    for k in ("read_id_map", "msa_len", "cells"):
+        if got[k] != want[k]:
+            return (None, k, None)
+    if got["msa"].shape != want["msa"].shape or not np.array_equal(got["msa"], want["msa"]):
+        return (None, "msa", None)
+    for a, (x, y) in enumerate(zip(got["alns"], want["alns"])):
+        for k in ("read_id", "qlen", "node_n", "best_score"):
+            if x[k] != y[k]:
+                return (a, k, None)
+        for k in ("cigar", "dp_beg", "dp_end"):
+            if len(x[k]) != len(y[k]):
+                return (a, k, "length %d vs %d" % (len(x[k]), len(y[k])))
+            bad = np.flatnonzero(np.asarray(x[k]) != np.asarray(y[k]))
+            if len(bad):
+                return (a, k, int(bad[0]))
+    if len(got["alns"]) != len(want["alns"]):
+        return (None, "alns", None)
+    return None
 
 
 class PoaParams:
@@ -427,6 +479,24 @@ class Engine:
                                                    cells.ctypes.data))
         msas = self._take_msas(outs, n_seq, ml)
         return (msas, cells[:n]) if return_cells else msas
+
+    def poa_msa_trace_batch(self, jobs, progressive=None):
+        """poa_msa_batch through the trace kernels: per job the dict of :func:`parse_trace` -- the MSA and cells, the read order,
+        and every alignment's read, query length, node count, best score, graph cigar and DP row bands as the device computed them."""
+        n_seq, lens, flat = self._pack(jobs)
+        n = len(jobs)
+        outs = (C.c_void_p * max(n, 1))()
+        nw = np.zeros(max(n, 1), np.int64)
+        prog = None if progressive is None else np.asarray(progressive, np.int32)
+        self._check(self.lib.barb200_poa_trace_batch(self.ctx, n, n_seq.ctypes.data, lens.ctypes.data, flat.ctypes.data,
+                                                     None if prog is None else prog.ctypes.data, outs, nw.ctypes.data))
+        res = []
+        for i in range(n):
+            k = int(nw[i])
+            w = np.ctypeslib.as_array(C.cast(outs[i], C.POINTER(C.c_int64)), shape=(k,)).copy()
+            self.lib.barb200_free(outs[i])
+            res.append(parse_trace(w, int(n_seq[i])))
+        return res
 
     def stage(self, jobs=None, packed=None, progressive=None):
         n_seq, lens, flat = packed if packed is not None else self._pack(jobs)

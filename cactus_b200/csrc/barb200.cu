@@ -21,11 +21,13 @@
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
+#include <deque>
 #include <functional>
 #include <memory>
 #include <mutex>
 #include <thread>
 #include <string>
+#include <unordered_map>
 #include <vector>
 #include "host_api.h"
 #include "poa_kernel.cuh"
@@ -38,17 +40,28 @@ extern "C" __global__ void poa_msa_kernel_t128(const BatchArgs A);
 extern "C" __global__ void poa_msa_kernel_t256(const BatchArgs A);
 extern "C" __global__ void poa_msa_kernel_t640(const BatchArgs A);
 extern "C" __global__ void poa_msa_kernel_t1024(const BatchArgs A);
+extern "C" __global__ void poa_trace_kernel_t32(const BatchArgs A, const TraceArgs T);
+extern "C" __global__ void poa_trace_kernel_t64(const BatchArgs A, const TraceArgs T);
+extern "C" __global__ void poa_trace_kernel_t128(const BatchArgs A, const TraceArgs T);
+extern "C" __global__ void poa_trace_kernel_t256(const BatchArgs A, const TraceArgs T);
+extern "C" __global__ void poa_trace_kernel_t640(const BatchArgs A, const TraceArgs T);
+extern "C" __global__ void poa_trace_kernel_t1024(const BatchArgs A, const TraceArgs T);
 }
 typedef void (*poa_kernel_fn)(const barb200::BatchArgs);
+typedef void (*poa_trace_kernel_fn)(const barb200::BatchArgs, const barb200::TraceArgs);
 // the kernel of every CTA-size class (stage_plan.h: kClassThreads), scratch = its dynamic shared memory per CTA
 // (poa_kernel.cuh: poa_scratch_bytes)
 static constexpr struct { int T; poa_kernel_fn fn; int scratch; } kKernels[] = {
     {32, barb200::poa_msa_kernel_t32, barb200::poa_scratch_bytes(32)}, {64, barb200::poa_msa_kernel_t64, barb200::poa_scratch_bytes(64)},
     {128, barb200::poa_msa_kernel_t128, barb200::poa_scratch_bytes(128)}, {256, barb200::poa_msa_kernel_t256, barb200::poa_scratch_bytes(256)},
     {640, barb200::poa_msa_kernel_t640, barb200::poa_scratch_bytes(640)}, {1024, barb200::poa_msa_kernel_t1024, barb200::poa_scratch_bytes(1024)}};
+// the trace kernels of the same classes (barb200_poa_trace_batch), with the same dynamic shared memory
+static constexpr poa_trace_kernel_fn kTraceKernels[] = {barb200::poa_trace_kernel_t32, barb200::poa_trace_kernel_t64, barb200::poa_trace_kernel_t128,
+                                                        barb200::poa_trace_kernel_t256, barb200::poa_trace_kernel_t640, barb200::poa_trace_kernel_t1024};
 static const int kNumKernels = barb200::kNumClasses;
 static constexpr bool kernels_follow_classes(int i = 0) { return i == kNumKernels || (kKernels[i].T == barb200::kClassThreads[i] && kernels_follow_classes(i + 1)); }
 static_assert(sizeof(kKernels) / sizeof(kKernels[0]) == kNumKernels && kernels_follow_classes(), "kKernels must follow stage_plan.h's classes");
+static_assert(sizeof(kTraceKernels) / sizeof(kTraceKernels[0]) == kNumKernels, "kTraceKernels must follow stage_plan.h's classes");
 static const int kMaxDevices = 8;
 using namespace barb200;
 
@@ -240,7 +253,10 @@ extern "C" barb200_ctx *barb200_create(const barb200_params *p, char *errbuf, in
         if (cudaGetDeviceProperties(&prop, ord) != cudaSuccess) { fail(errbuf, errbuf_len, "cudaGetDeviceProperties failed"); barb200_destroy(ctx.release()); return nullptr; }
         std::unique_ptr<Device> D(new Device());
         D->ordinal = ord; D->sm_count = prop.multiProcessorCount; D->mem_total = prop.totalGlobalMem;
-        for (int i = 0; i < kNumKernels; ++i) cudaFuncSetAttribute(kKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kKernels[i].scratch);
+        for (int i = 0; i < kNumKernels; ++i) {
+            cudaFuncSetAttribute(kKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kKernels[i].scratch);
+            cudaFuncSetAttribute(kTraceKernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kKernels[i].scratch);
+        }
         bool ok = true;
         for (int l = 0; l < ctx->lanes_per_device && ok; ++l) {
             std::unique_ptr<Lane> L(new Lane());
@@ -337,6 +353,7 @@ struct barb200_stage {
     JobDesc *d_desc = nullptr; int *d_msa_len = nullptr, *d_status = nullptr, *d_next = nullptr; long long *d_cells = nullptr;
     int *d_order = nullptr, *d_gt_status = nullptr; uint8_t *d_gt_scratch = nullptr;
     GuideTreeArgs gt; cudaEvent_t e_gt = nullptr;                    // K0: the guide trees of the stage (guide_tree.cu)
+    TraceArgs trace{};                                               // a trace stage's regions (plan.trace)
     std::vector<int> status;                                         // of the last run
     std::vector<std::unique_ptr<barb200_stage>> retries;             // the last run's capacity retries: x4, then worst case
     int64_t launches = 0; bool ran = false;
@@ -367,7 +384,8 @@ static int plan_stage(barb200_stage *st) {
         // never below the sweep's ring, which the kernel uses without a run-time check (the topological sort and the MSA ranking
         // fit whatever is left, falling back to global memory)
         smem = std::max(smem, (size_t)poa_ring_bytes(B.T));
-        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[b], kKernels[B.cls].fn, B.T, smem));
+        if (st->plan.trace) CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[b], kTraceKernels[B.cls], B.T, smem));
+        else CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[b], kKernels[B.cls].fn, B.T, smem));
         if (per_sm[b] < 1) { set_error(ctx, "kernel does not fit on an SM with the requested configuration"); return BARB200_EINVAL; }
         if (ctx->p.ctas_per_sm > 0) per_sm[b] = std::min(per_sm[b], ctx->p.ctas_per_sm);
         st->dyn_smem[b] = smem;
@@ -417,10 +435,18 @@ static int ensure_arena(barb200_ctx *ctx, Device &D, Lane &LN, size_t slots_byte
 static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 static bool timing_on() { static const bool on = getenv("BARB200_TIMING") != nullptr; return on; }
 
+// BARB200_TRACE_REGION_SCALE (test aid, read at every stage): a factor on a trace stage's regions below the worst case, so that a test
+// can make them overflow on any input (the kernel's capacity check, JOB_ERR_TRACE_CAP and its retries)
+static double trace_region_scale() {
+    const char *v = getenv("BARB200_TRACE_REGION_SCALE");
+    return v ? std::max(0.0, atof(v)) : 1.0;
+}
+
 // A stage over the table's jobs `jobs` (caller indices); grow / worst_case size the slots (capacity-miss retries). A call's first
-// stage uploads the table's bases from `seqs`; a retry runs on its first stage's device copy `d_seqs` and uploads none.
+// stage uploads the table's bases from `seqs`; a retry runs on its first stage's device copy `d_seqs` and uploads none. trace: the
+// stage runs the trace kernels (barb200_poa_trace_batch).
 static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTable> tab, std::vector<int64_t> jobs, double grow, bool worst_case,
-                       const uint8_t *seqs, uint8_t *d_seqs, barb200_stage **out) {
+                       const uint8_t *seqs, uint8_t *d_seqs, barb200_stage **out, bool trace = false) {
     Device &D = dev_of_lane(ctx, lane);
     Lane &LN = lane_of(ctx, lane);
     cudaSetDevice(D.ordinal);
@@ -428,7 +454,8 @@ static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTabl
     const int64_t n_jobs = (int64_t)jobs.size();
     st->ctx = ctx; st->lane = lane; st->tab = std::move(tab); st->n_jobs = n_jobs;
     const double tb0 = now_ms();
-    const StagePlan &S = st->plan = plan_stage_order(*st->tab, std::move(jobs), ctx->p, grow, worst_case, D.sm_count, d_seqs == nullptr);
+    const StagePlan &S = st->plan = plan_stage_order(*st->tab, std::move(jobs), ctx->p, grow, worst_case, D.sm_count, d_seqs == nullptr, trace,
+                                                     trace ? trace_region_scale() : 1.0);
     if (n_jobs == 0) { *out = st.release(); return BARB200_OK; }
     const double tb2 = now_ms();
     int rc = plan_stage(st.get());
@@ -445,6 +472,10 @@ static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTabl
     st->d_desc = (JobDesc *)(blk + S.o_desc); st->d_msa = blk + S.o_msa; st->d_msa_len = (int *)(blk + S.o_msa_len); st->d_status = (int *)(blk + S.o_status);
     st->d_cells = (long long *)(blk + S.o_cells); st->d_next = (int *)(blk + S.o_next);
     st->d_order = (int *)(blk + S.o_order); st->d_gt_status = (int *)(blk + S.o_gt_status); st->d_gt_scratch = blk + S.o_gt_scratch;
+    if (S.trace) {
+        st->trace.words = (int64_t *)(blk + S.o_trace); st->trace.off = (const int64_t *)(blk + S.o_trace_off);
+        st->trace.cap = (const int64_t *)(blk + S.o_trace_cap); st->trace.used = (int64_t *)(blk + S.o_trace_used);
+    }
     GuideTreeArgs &GA = st->gt;
     memset(&GA, 0, sizeof(GA));
     GA.jobs = st->d_desc; GA.n_jobs = (int)n_jobs; GA.seqs = st->d_seqs; GA.lens = st->d_lens; GA.soff = st->d_soff; GA.order = st->d_order; GA.gt_status = st->d_gt_status;
@@ -456,6 +487,8 @@ static int stage_build(barb200_ctx *ctx, int lane, std::shared_ptr<const JobTabl
         (e = cudaMemcpyAsync(st->d_lens, S.lens.data(), ns * 4, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaMemcpyAsync(st->d_soff, S.soff.data(), ns * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess ||
         (e = cudaMemcpyAsync(st->d_desc, S.desc.data(), n_jobs * sizeof(JobDesc), cudaMemcpyHostToDevice, s)) != cudaSuccess ||
+        (S.trace && (e = cudaMemcpyAsync((void *)st->trace.off, S.trace_off.data(), n_jobs * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess) ||
+        (S.trace && (e = cudaMemcpyAsync((void *)st->trace.cap, S.trace_cap.data(), n_jobs * 8, cudaMemcpyHostToDevice, s)) != cudaSuccess) ||
         (e = cudaStreamSynchronize(s)) != cudaSuccess) {
         set_error(ctx, std::string("H2D failed: ") + cudaGetErrorString(e)); return BARB200_ECUDA;
     }
@@ -510,11 +543,15 @@ static int stage_launch(barb200_stage *st) {
         A.slots = LN.d_slots + B.slot_off; A.planes = LN.d_planes + B.plane_off; A.next_job = st->d_next + b;
         A.phase_clk = clk_n ? LN.d_clk + B.clk_off : nullptr;
         A.serial_phases = getenv("BARB200_DEBUG_SERIAL") ? 1 : 0;
-        A.bfs_order = getenv("BARB200_DEBUG_BFS") ? 1 : 0;
+        // a trace stage numbers its rows as abPOA does (the BFS order after every fusion): the splice's order is an equally valid
+        // topological order with the same DP values per node, but other row indices, and the trace compares bands row by row. So a
+        // trace does not run the production kernels' splice order, nor the far-row paths that order gives the sweep
+        A.bfs_order = (S.trace || getenv("BARB200_DEBUG_BFS")) ? 1 : 0;
         A.scratch_bytes = (int)st->dyn_smem[b]; A.lay = B.lay; A.P = ctx->P;
         cudaStream_t cs = single ? s : LN.cls[B.cls];
         if (!single) CUDA_TRY(ctx, cudaStreamWaitEvent(cs, st->e_gt, 0));
-        kKernels[B.cls].fn<<<B.slots, B.T, st->dyn_smem[b], cs>>>(A);
+        if (S.trace) kTraceKernels[B.cls]<<<B.slots, B.T, st->dyn_smem[b], cs>>>(A, st->trace);
+        else kKernels[B.cls].fn<<<B.slots, B.T, st->dyn_smem[b], cs>>>(A);
         cudaError_t le = cudaGetLastError();
         if (le != cudaSuccess) { set_error(ctx, std::string("kernel launch: ") + cudaGetErrorString(le)); return BARB200_ECUDA; }
         if (!single) { CUDA_TRY(ctx, cudaEventRecord(LN.cls_done[B.cls], cs)); CUDA_TRY(ctx, cudaStreamWaitEvent(s, LN.cls_done[B.cls], 0)); }
@@ -540,6 +577,7 @@ static int stage_finish(barb200_stage *st, float *kernel_ms) {
     cudaStream_t s = LN.main;
     float ms = 0.f;
     for (int k = 0; k < 7; ++k) st->clk[k] = 0;
+    std::deque<RetryRound> pending;                  // retry stages still to run
     for (barb200_stage *r = st;;) {
         cudaError_t se = cudaStreamSynchronize(s);
         if (se != cudaSuccess) { set_error(ctx, std::string("kernel execution: ") + cudaGetErrorString(se)); return BARB200_ECUDA; }
@@ -557,13 +595,18 @@ static int stage_finish(barb200_stage *st, float *kernel_ms) {
             CUDA_TRY(ctx, cudaMemcpy(h.data(), LN.d_clk, clk_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
             for (size_t b = 0; b < clk_n / PH_N; ++b) for (int k = 0; k < 6; ++k) st->clk[k] += h[b * PH_N + k];
         }
-        // capacity misses -> retry launch for just those jobs with larger slots (x4 first, then worst case)
+        // capacity misses -> retry launch for just those jobs with larger slots (x4 first, then worst case); a trace stage's retry may
+        // be cut into several stages (retry_batches), which run one after the other
         RetryRound next;
         const std::string err = retry_round(r->plan, r->status, next);
         if (!err.empty()) { set_error(ctx, err); return BARB200_EJOB; }
-        if (next.jobs.empty()) break;
+        if (!next.jobs.empty())
+            for (std::vector<int64_t> &b : retry_batches(*st->tab, r->plan, next)) pending.push_back(RetryRound{std::move(b), next.grow, next.worst_case});
+        if (pending.empty()) break;
+        RetryRound todo = std::move(pending.front());
+        pending.pop_front();
         barb200_stage *rs = nullptr;
-        int rc = stage_build(ctx, st->lane, st->tab, std::move(next.jobs), next.grow, next.worst_case, nullptr, st->d_seqs, &rs);
+        int rc = stage_build(ctx, st->lane, st->tab, std::move(todo.jobs), todo.grow, todo.worst_case, nullptr, st->d_seqs, &rs, st->plan.trace);
         if (rc) return rc;
         st->retries.emplace_back(rs);
         if ((rc = stage_launch(rs))) return rc;
@@ -685,16 +728,12 @@ static int batch_on_lane(barb200_ctx *ctx, int lane, const std::shared_ptr<const
     return rc;
 }
 
-extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens,
-                                     const uint8_t *seqs, const int *progressive, uint8_t **msa_out, int *msa_len,
-                                     int64_t *cells) {
-    if (!ctx) return BARB200_EINVAL;
-    if (msa_out) for (int64_t j = 0; j < n_jobs; ++j) msa_out[j] = nullptr;
-    auto tab = std::make_shared<JobTable>();
-    const int trc = table_rc(ctx, table_of_arrays(ctx->p, host_threads(ctx), n_jobs, n_seq, seq_lens, seqs, progressive, *tab));
-    if (trc || n_jobs == 0) return trc;
+// The table's jobs dealt over the context's devices (deal_jobs); each device's share is cut into device batches (chunk_ends, with
+// trace_words for a trace call) that run(lane, jobs) runs one after the other on the device's first lane, the devices in parallel.
+// Returns BARB200_OK or the code of a failed device, with that device's message.
+static int run_dealt(barb200_ctx *ctx, const JobTable &tab, int64_t trace_words, const std::function<int(int, std::vector<int64_t>)> &run) {
     const int ndev = (int)ctx->devs.size();
-    const std::vector<std::vector<int64_t>> share = deal_jobs(*tab, ndev);
+    const std::vector<std::vector<int64_t>> share = deal_jobs(tab, ndev);
     std::vector<int> rcs(ndev, BARB200_OK);
     std::vector<std::string> errs(ndev);
     int active_devs = 0;
@@ -705,8 +744,8 @@ extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int
         const int lane = d * ctx->lanes_per_device;
         std::lock_guard<std::mutex> lk(lane_of(ctx, lane).busy);
         size_t at = 0;
-        for (size_t end : chunk_ends(*tab, mine)) {
-            const int rc = batch_on_lane(ctx, lane, tab, std::vector<int64_t>(mine.begin() + at, mine.begin() + end), seqs, malloc_dest(msa_out), msa_len, cells);
+        for (size_t end : chunk_ends(tab, mine, trace_words)) {
+            const int rc = run(lane, std::vector<int64_t>(mine.begin() + at, mine.begin() + end));
             if (rc) { rcs[d] = rc; errs[d] = get_error(ctx); break; }
             at = end;
         }
@@ -717,11 +756,84 @@ extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int
         for (int d = 0; d < ndev; ++d) if (!share[d].empty()) th.emplace_back(run_device, d);
         for (auto &t : th) t.join();
     }
-    for (int d = 0; d < ndev; ++d) if (rcs[d]) {
-        if (msa_out) for (int64_t j = 0; j < n_jobs; ++j) { free(msa_out[j]); msa_out[j] = nullptr; }
-        set_error(ctx, errs[d]); return rcs[d];
-    }
+    for (int d = 0; d < ndev; ++d) if (rcs[d]) { set_error(ctx, errs[d]); return rcs[d]; }
     return BARB200_OK;
+}
+
+extern "C" int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens,
+                                     const uint8_t *seqs, const int *progressive, uint8_t **msa_out, int *msa_len,
+                                     int64_t *cells) {
+    if (!ctx) return BARB200_EINVAL;
+    if (msa_out) for (int64_t j = 0; j < n_jobs; ++j) msa_out[j] = nullptr;
+    auto tab = std::make_shared<JobTable>();
+    const int trc = table_rc(ctx, table_of_arrays(ctx->p, host_threads(ctx), n_jobs, n_seq, seq_lens, seqs, progressive, *tab));
+    if (trc || n_jobs == 0) return trc;
+    const int rc = run_dealt(ctx, *tab, 0, [&](int lane, std::vector<int64_t> jobs) {
+        return batch_on_lane(ctx, lane, tab, std::move(jobs), seqs, malloc_dest(msa_out), msa_len, cells);
+    });
+    if (rc && msa_out) for (int64_t j = 0; j < n_jobs; ++j) { free(msa_out[j]); msa_out[j] = nullptr; }
+    return rc;
+}
+
+// One device batch of a trace call on one lane (the caller holds the lane): the trace kernels' stage and its capacity retries, then
+// every job's word array (include/barb200.h) from the round that completed it -- header, read order, the kernel's records, the MSA.
+// cells: per caller job, filled on the way.
+static int trace_batch_on_lane(barb200_ctx *ctx, int lane, const std::shared_ptr<const JobTable> &tab, std::vector<int64_t> jobs, const uint8_t *seqs,
+                               int64_t **trace_out, int64_t *n_words, int64_t *cells) {
+    barb200_stage *stp = nullptr;
+    int rc = stage_build(ctx, lane, tab, std::move(jobs), 1.0, false, seqs, nullptr, &stp, true);
+    if (rc) return rc;
+    std::unique_ptr<barb200_stage> st(stp);
+    if ((rc = stage_launch(st.get())) || (rc = stage_finish(st.get(), nullptr))) return rc;
+    if (st->n_jobs == 0) return BARB200_OK;
+    // the records and read orders of every round, and where each caller job's are
+    std::vector<barb200_stage *> rounds{st.get()};
+    for (auto &r : st->retries) rounds.push_back(r.get());
+    std::vector<std::vector<int64_t>> words(rounds.size()), used(rounds.size());
+    std::vector<std::vector<int>> order(rounds.size());
+    struct Done { const int64_t *rec; int64_t n; const int *order; };
+    std::unordered_map<int64_t, Done> done;
+    cudaStream_t s = lane_of(ctx, lane).main;
+    for (size_t k = 0; k < rounds.size(); ++k) {
+        barb200_stage *r = rounds[k];
+        words[k].resize(r->plan.trace_words); used[k].resize(r->n_jobs); order[k].resize(r->plan.n_seqs);
+        CUDA_TRY(ctx, cudaMemcpyAsync(words[k].data(), r->trace.words, words[k].size() * 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaMemcpyAsync(used[k].data(), r->trace.used, used[k].size() * 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaMemcpyAsync(order[k].data(), r->d_order, order[k].size() * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        for (int64_t j = 0; j < r->n_jobs; ++j)
+            if (r->status[j] == JOB_OK) done[r->plan.perm[j]] = Done{words[k].data() + r->plan.trace_off[j], used[k][j], order[k].data() + r->plan.desc[j].len_off};
+    }
+    // the MSA lands behind the records: stage_fetch_locked writes its K rows of msa_len bytes back to back where dest points
+    const MsaDest dest = [&](int64_t c, int K, int ml) -> uint8_t * {
+        const Done &D = done.at(c);
+        const int64_t msa_words = ((int64_t)K * ml + 7) / 8, n = 3 + K + D.n + msa_words;
+        int64_t *w = (int64_t *)malloc((size_t)n * 8);
+        if (!w) return nullptr;
+        w[0] = K; w[1] = ml; w[2] = cells[c];
+        for (int i = 0; i < K; ++i) w[3 + i] = D.order[i];
+        memcpy(w + 3 + K, D.rec, (size_t)D.n * 8);
+        if (msa_words) w[n - 1] = 0;
+        trace_out[c] = w; n_words[c] = n;
+        return (uint8_t *)(w + 3 + K + D.n);
+    };
+    return stage_fetch_locked(st.get(), dest, nullptr, cells);
+}
+
+extern "C" int barb200_poa_trace_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs,
+                                       const int *progressive, int64_t **trace_out, int64_t *n_words) {
+    if (!ctx) return BARB200_EINVAL;
+    if (n_jobs > 0 && (!trace_out || !n_words)) { set_error(ctx, "bad arguments"); return BARB200_EINVAL; }
+    for (int64_t j = 0; j < n_jobs; ++j) { trace_out[j] = nullptr; n_words[j] = 0; }
+    auto tab = std::make_shared<JobTable>();
+    const int trc = table_rc(ctx, table_of_arrays(ctx->p, host_threads(ctx), n_jobs, n_seq, seq_lens, seqs, progressive, *tab));
+    if (trc || n_jobs == 0) return trc;
+    std::vector<int64_t> cells(n_jobs, 0);
+    const int rc = run_dealt(ctx, *tab, kMaxTraceWordsPerBatch, [&](int lane, std::vector<int64_t> jobs) {
+        return trace_batch_on_lane(ctx, lane, tab, std::move(jobs), seqs, trace_out, n_words, cells.data());
+    });
+    if (rc) for (int64_t j = 0; j < n_jobs; ++j) { free(trace_out[j]); trace_out[j] = nullptr; n_words[j] = 0; }
+    return rc;
 }
 
 // host-side phases of the most recent device batch, milliseconds: out[0] build (ordering, planning, H2D), out[1] launch +

@@ -31,6 +31,7 @@
 // are bit-identical to abPOA's AVX2 path.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "poa_graph.cuh"
 #include "poa_cta.cuh"
 #include "poa_kernel.cuh"
@@ -447,10 +448,43 @@ __device__ long long dp_sweep(KShared &S, const BatchArgs &A, const uint8_t *__r
 
 #define PHASE_TICK(ph) do { if (A.phase_clk && threadIdx.x == 0) { unsigned long long _n = clock64(); A.phase_clk[(size_t)blockIdx.x * PH_N + (ph)] += _n - t_last; t_last = _n; } } while (0)
 
-template <int NT>
-__device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
+// ---- the trace kernels' per-alignment record (TraceArgs, poa_kernel.cuh; word layout in include/barb200.h) --------------------
+// The shared state of a trace kernel: the production kernels' plus the job's next free word in its trace region.
+struct KSharedTrace : KShared { int64_t trace_pos; };
+
+// One alignment's record, appended to the job's trace region by the whole CTA after the traceback and before the fusion: read id,
+// query length, node_n before the alignment, cigar length, best score, rows (node_n - 1; 0 for the first read, which is not
+// aligned), the cigar, then dp_beg and dp_end of every row. A record that does not fit the region is not written: the job ends with
+// JOB_ERR_TRACE_CAP (the host retries it with a larger region). Called by every thread of the CTA; S.g.err is read before the first
+// barrier and written only after it.
+__device__ void trace_record(KSharedTrace &S, const TraceArgs &T, int job, int read, int L, bool aligned) {
+    const int tid = threadIdx.x;
+    const int n_rows = aligned ? S.g.node_n - 1 : 0, nc = aligned ? S.d.n_cigar : 0, node_n = S.g.node_n;
+    const int64_t size = 6 + nc + 2 * (int64_t)n_rows, pos = S.trace_pos;
+    const bool ok = !S.g.err && pos + size <= T.cap[job];
+    const bool full = !S.g.err && !ok;
+    __syncthreads();
+    if (ok) {
+        int64_t *w = T.words + T.off[job] + pos;
+        const int64_t hdr = tid == 0 ? read : tid == 1 ? L : tid == 2 ? node_n : tid == 3 ? nc : tid == 4 ? (aligned ? S.d.best_score : 0) : n_rows;
+        if (tid < 6) w[tid] = hdr;
+        const uint64_t *cg = S.d.cigar;
+        for (int k = tid; k < nc; k += blockDim.x) w[6 + k] = (int64_t)cg[k];
+        const RowInfo *info = S.d.info;
+        int64_t *wb = w + 6 + nc;
+        for (int r = tid; r < n_rows; r += blockDim.x) { const RowInfo ri = info[r]; wb[r] = ri.beg; wb[n_rows + r] = ri.end; }
+    }
+    if (full && tid == 0) S.g.err = JOB_ERR_TRACE_CAP;
+    __syncthreads();
+    if (ok && tid == 0) S.trace_pos = pos + size;
+}
+
+// TRACE: the trace kernels (poa_trace_kernel_t*), which also write every alignment's record to TA; the production kernels
+// (poa_msa_kernel_t*) instantiate TRACE = false and compile to the code they had before the trace kernels existed
+template <int NT, bool TRACE>
+__device__ __forceinline__ void poa_msa_body(const BatchArgs &A, const TraceArgs *TA) {
     extern __shared__ __align__(16) unsigned char dyn_smem[];    // scratch of the topological sort (poa_cta.cuh), the sweep's row ring
-    __shared__ KShared S;
+    __shared__ std::conditional_t<TRACE, KSharedTrace, KShared> S;
     __shared__ uint4 qsm[NT];                                    // query codes of each thread's columns (dp_sweep)
     const int tid = threadIdx.x;
     int *ws = &S.wF[0][0][0];
@@ -476,7 +510,10 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
         const int *lens = A.lens + jd.len_off;
         const int64_t *soff = A.soff + jd.len_off;
         const uint8_t *seqs = A.seqs + jd.seq_off;
-        if (tid == 0) { graph_reset(S.g, K); S.abort_s = 0; }
+        if (tid == 0) {
+            graph_reset(S.g, K); S.abort_s = 0;
+            if constexpr (TRACE) S.trace_pos = 0;
+        }
         __syncthreads();
         // read order: the job's guide tree (abpoa_seed.c:705-722), computed by guide_tree_kernel before this launch (guide_tree.cu)
         const int *const order = A.order + jd.len_off;
@@ -487,6 +524,7 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
             const int read = order[a], L = lens[read];
             const uint8_t *q = seqs + soff[read];
             if (a == 0) {
+                if constexpr (TRACE) trace_record(S, *TA, job, read, L, false);
                 if (A.serial_phases) { if (tid == 0) graph_add_first_sequence(S.g, q, L, read); }
                 else cta_add_first_sequence(S.g, q, L, read);
                 PHASE_TICK(PH_FUSE);
@@ -501,6 +539,7 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
                 else if (tid < 32 && !S.g.err) warp_backtrack(S.g, S.rt, S.d, A.P, S.smat, q, L);
                 PHASE_TICK(PH_BACKTRACK);
                 __syncthreads();
+                if constexpr (TRACE) trace_record(S, *TA, job, read, L, true);
                 if (A.serial_phases) { if (tid == 0 && !S.g.err) graph_fuse_alignment(S.g, q, S.d.cigar, S.d.n_cigar, read); }
                 else if (!S.g.err) cta_fuse_alignment(S.g, q, L, S.d.cigar, S.d.n_cigar, read, ws, dyn_smem, A.scratch_bytes);
                 PHASE_TICK(PH_FUSE);
@@ -529,24 +568,39 @@ __device__ __forceinline__ void poa_msa_body(const BatchArgs &A) {
         }
         __syncthreads();
         if (tid == 0) { A.status[job] = S.g.err; A.msa_len[job] = S.g.err ? 0 : S.msa_len_s; A.cells[job] = cells; }
+        if constexpr (TRACE) { if (tid == 0) TA->used[job] = S.g.err ? 0 : S.trace_pos; }
         PHASE_TICK(PH_MSA);
         __syncthreads();
     }
     if (A.phase_clk && tid == 0) A.phase_clk[(size_t)blockIdx.x * PH_N + PH_TOTAL] += clock64() - t_start;
 }
 
+#ifndef BARB200_T128_MINB
+#define BARB200_T128_MINB 4
+#endif
+#ifndef BARB200_TRACE_KERNELS
 // One entry point per CTA-size class (the register budget per thread follows from the launch bounds):
 //   queries up to 511 bases -> one warp, 16 CTAs per SM;  up to 1023 -> 64 threads;
 //   up to 2047 -> 128 threads, 4 CTAs per SM;  up to 4095 -> 256 threads, 2 per SM;
 //   up to 10239 (covers Cactus' 10 kbp window) -> 640 threads;  up to 16383 -> 1024 threads.
-extern "C" __global__ void __launch_bounds__(32, 16) poa_msa_kernel_t32(const BatchArgs A) { poa_msa_body<32>(A); }
-extern "C" __global__ void __launch_bounds__(64, 8) poa_msa_kernel_t64(const BatchArgs A) { poa_msa_body<64>(A); }
-#ifndef BARB200_T128_MINB
-#define BARB200_T128_MINB 4
+extern "C" __global__ void __launch_bounds__(32, 16) poa_msa_kernel_t32(const BatchArgs A) { poa_msa_body<32, false>(A, nullptr); }
+extern "C" __global__ void __launch_bounds__(64, 8) poa_msa_kernel_t64(const BatchArgs A) { poa_msa_body<64, false>(A, nullptr); }
+extern "C" __global__ void __launch_bounds__(128, BARB200_T128_MINB) poa_msa_kernel_t128(const BatchArgs A) { poa_msa_body<128, false>(A, nullptr); }
+extern "C" __global__ void __launch_bounds__(256, 2) poa_msa_kernel_t256(const BatchArgs A) { poa_msa_body<256, false>(A, nullptr); }
+extern "C" __global__ void __launch_bounds__(640, 1) poa_msa_kernel_t640(const BatchArgs A) { poa_msa_body<640, false>(A, nullptr); }
+extern "C" __global__ void __launch_bounds__(1024, 1) poa_msa_kernel_t1024(const BatchArgs A) { poa_msa_body<1024, false>(A, nullptr); }
+
+#else
+// The trace kernels (barb200_poa_trace_batch): the same classes and launch bounds, plus every alignment's record. They are compiled
+// in a module of their own (poa_trace_kernel.cu defines BARB200_TRACE_KERNELS and includes this file): NVVM's code for a kernel
+// depends on the other functions of its module, and next to the trace kernels the 10 kbp class came out scheduled differently. Not
+// named poa_msa_kernel_t*, so that the SASS checks of the production kernels see only those.
+extern "C" __global__ void __launch_bounds__(32, 16) poa_trace_kernel_t32(const BatchArgs A, const TraceArgs T) { poa_msa_body<32, true>(A, &T); }
+extern "C" __global__ void __launch_bounds__(64, 8) poa_trace_kernel_t64(const BatchArgs A, const TraceArgs T) { poa_msa_body<64, true>(A, &T); }
+extern "C" __global__ void __launch_bounds__(128, BARB200_T128_MINB) poa_trace_kernel_t128(const BatchArgs A, const TraceArgs T) { poa_msa_body<128, true>(A, &T); }
+extern "C" __global__ void __launch_bounds__(256, 2) poa_trace_kernel_t256(const BatchArgs A, const TraceArgs T) { poa_msa_body<256, true>(A, &T); }
+extern "C" __global__ void __launch_bounds__(640, 1) poa_trace_kernel_t640(const BatchArgs A, const TraceArgs T) { poa_msa_body<640, true>(A, &T); }
+extern "C" __global__ void __launch_bounds__(1024, 1) poa_trace_kernel_t1024(const BatchArgs A, const TraceArgs T) { poa_msa_body<1024, true>(A, &T); }
 #endif
-extern "C" __global__ void __launch_bounds__(128, BARB200_T128_MINB) poa_msa_kernel_t128(const BatchArgs A) { poa_msa_body<128>(A); }
-extern "C" __global__ void __launch_bounds__(256, 2) poa_msa_kernel_t256(const BatchArgs A) { poa_msa_body<256>(A); }
-extern "C" __global__ void __launch_bounds__(640, 1) poa_msa_kernel_t640(const BatchArgs A) { poa_msa_body<640>(A); }
-extern "C" __global__ void __launch_bounds__(1024, 1) poa_msa_kernel_t1024(const BatchArgs A) { poa_msa_body<1024>(A); }
 
 }  // namespace barb200

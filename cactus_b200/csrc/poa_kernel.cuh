@@ -37,6 +37,15 @@ struct BatchArgs {
     PoaParams P;
 };
 
+// The trace kernels' output (poa_trace_kernel_t*, barb200_poa_trace_batch): per job of the stage (internal order), a region of
+// `words` where every alignment appends its record (poa_kernel.cu: trace_record). Capacities: slot_plan.h, trace_words_for_job.
+struct TraceArgs {
+    int64_t *words;             // the stage's trace buffer
+    const int64_t *off;         // per job: first word of its region
+    const int64_t *cap;         // per job: words in its region
+    int64_t *used;              // out, per job: words written (0 if the job failed)
+};
+
 // ---- K0: guide_tree_kernel (guide_tree.cu): the read order of every job of a stage, one persistent CTA per scratch slot ----
 struct GuideTreeArgs {
     const JobDesc *jobs; int n_jobs;

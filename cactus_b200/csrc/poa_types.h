@@ -44,7 +44,8 @@ enum JobStatus : int {
     JOB_ERR_BACKTRACK = 7,   // "Error in cg_backtrack" in the reference (abpoa_align_simd.c:448)
     JOB_ERR_ALIGNED_CAP = 8,
     JOB_ERR_QUERY_LEN = 9,   // query longer than 16 x threads per CTA (host sizing bug)
-    JOB_ERR_GT_CAP = 10      // minimizer keys of the guide tree outgrew the slot (host retries with a larger slot)
+    JOB_ERR_GT_CAP = 10,     // minimizer keys of the guide tree outgrew the slot (host retries with a larger slot)
+    JOB_ERR_TRACE_CAP = 11   // a trace kernel's alignment records outgrew the job's trace region (host retries with a larger one)
 };
 
 // Scoring / banding parameters: what abpoaParamaters_constructFromCactusParams builds

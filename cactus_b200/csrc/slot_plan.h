@@ -133,16 +133,31 @@ HD GtScratch gt_views(const GtLayout &Y, uint8_t *b) {
 // however far the best columns of the predecessors have drifted from the row's diagonal d; a quarter of 2w is allowed for that
 // before the geometric retries take over. Only windows longer than ~2.5 kbp are narrower than the whole row (w = 1000 + 0.1 L):
 // a 10 kbp window plans 0.77 GB of planes instead of 1.53 GB.
+// Optimistic rows of a job's graph: the longest read plus an eighth of the other bases, plus a margin.
+inline int64_t optimistic_rows(int64_t sum, int64_t ml) { return ml + (sum - ml) / 8 + 256; }
+
 inline int64_t plane_ints_for_job(int wb, double wf, int64_t K, int64_t sum, int64_t ml, double grow, bool worst_case) {
     (void)K;
     int64_t rows = sum + 2;
-    if (!worst_case) rows = std::min<int64_t>(rows, (int64_t)(grow * (double)(ml + (sum - ml) / 8 + 256)));
+    if (!worst_case) rows = std::min<int64_t>(rows, (int64_t)(grow * (double)optimistic_rows(sum, ml)));
     int64_t width = ml + 1;
     if (!worst_case) {
         const int64_t w = (int64_t)wb + (int64_t)(wf * (double)ml);
         width = std::min<int64_t>(width, (int64_t)(grow * (2.5 * (double)w + 64.0)));
     }
     return rows * (TB / CPT) * ((width + CPT - 1) / CPT * CPT + CPT);
+}
+
+// Words of a job's trace region (the trace kernels, poa_kernel.cu: trace_record): K records of 6 header words, the cigar and two
+// words per row. At the worst case from the bounds of a slot planned for the job alone: rows = node_n - 1 < node_cap, and a cigar
+// holds at most cigar_cap ops (the traceback fails the job beyond that). Optimistic: plane_ints_for_job's row estimate for every
+// alignment, and a cigar of one op per query base and row; grow: the capacity retries, as for the planes.
+inline int64_t trace_words_for_job(int64_t K, int64_t sum, int64_t ml, double grow, bool worst_case) {
+    const int64_t node_cap = sum + 2, cigar_cap = ml + node_cap + 16;   // plan_slot of SlotNeeds::add_job(K, sum, ml, ...)
+    const int64_t worst = K * (6 + cigar_cap + 2 * node_cap);
+    if (worst_case) return worst;
+    const int64_t rows = optimistic_rows(sum, ml);
+    return std::min<int64_t>(worst, (int64_t)(grow * (double)(K * (6 + ml + 3 * rows))));
 }
 
 // Device bytes a lane may plan a stage with: a fraction of what is free plus what the lane's arena already holds, minus the

@@ -126,14 +126,21 @@ struct StagePlan {
     int64_t o_seqs = 0, o_lens = 0, o_soff = 0, o_desc = 0, o_msa = 0, o_msa_len = 0, o_status = 0, o_cells = 0, o_next = 0, o_order = 0, o_gt_status = 0, o_gt_scratch = 0, block_bytes = 0;
     // set by fit_stage: the lane arena the buckets take
     size_t slots_bytes = 0, plane_ints = 0, clk_entries = 0;
+    // a trace stage (barb200_poa_trace_batch): per job its region of the trace buffer (first word, words; trace_words_for_job), and
+    // the byte offsets of the buffer, the two tables and the words each job wrote in the stage's block
+    bool trace = false;
+    std::vector<int64_t> trace_off, trace_cap;
+    int64_t trace_words = 0, o_trace = 0, o_trace_off = 0, o_trace_cap = 0, o_trace_used = 0;
 };
 
 // The stage over the table's jobs `jobs` (caller indices) sized for (grow, worst_case), on a device of sm_count SMs; own_seqs:
-// its block holds the table's bases (a capacity retry reads its first stage's). Slot layouts are planned; slots are fit_stage's.
+// its block holds the table's bases (a capacity retry reads its first stage's); trace: the stage runs the trace kernels, and its block
+// holds every job's trace region; trace_scale scales the regions below the worst case (a test aid that makes them overflow: the
+// kernel's capacity check and the trace-capacity retries then run on any input). Slot layouts are planned; slots are fit_stage's.
 inline StagePlan plan_stage_order(const JobTable &T, std::vector<int64_t> jobs, const barb200_params &p, double grow, bool worst_case, int sm_count,
-                                  bool own_seqs) {
+                                  bool own_seqs, bool trace = false, double trace_scale = 1.0) {
     StagePlan S;
-    S.grow = grow; S.worst_case = worst_case;
+    S.grow = grow; S.worst_case = worst_case; S.trace = trace;
     const int64_t n_jobs = (int64_t)jobs.size();
     S.perm = std::move(jobs);
     std::stable_sort(S.perm.begin(), S.perm.end(), [&](int64_t a, int64_t b) {
@@ -177,6 +184,17 @@ inline StagePlan plan_stage_order(const JobTable &T, std::vector<int64_t> jobs, 
     S.o_seqs = own_seqs ? sub.take(T.n_bases) : 0; S.o_lens = sub.take(ns * 4); S.o_soff = sub.take(ns * 8); S.o_desc = sub.take(n_jobs * sizeof(JobDesc));
     S.o_msa = sub.take(S.msa_bytes); S.o_msa_len = sub.take(n_jobs * 4); S.o_status = sub.take(n_jobs * 4); S.o_cells = sub.take(n_jobs * 8);
     S.o_next = sub.take(4 * (kNumClasses + 1)); S.o_order = sub.take(ns * 4); S.o_gt_status = sub.take(n_jobs * 4); S.o_gt_scratch = sub.take(S.gt.slot_bytes * S.gt_ctas);
+    if (trace) {
+        S.trace_off.resize(n_jobs); S.trace_cap.resize(n_jobs);
+        for (int64_t j = 0; j < n_jobs; ++j) {
+            const TableJob &J = T.jobs[S.perm[j]];
+            int64_t cap = trace_words_for_job(J.n_seq, J.sum_len, J.max_len, grow, worst_case);
+            if (!worst_case) cap = std::min(cap, (int64_t)(trace_scale * (double)cap));
+            S.trace_off[j] = S.trace_words; S.trace_cap[j] = cap;
+            S.trace_words += S.trace_cap[j];
+        }
+        S.o_trace = sub.take(S.trace_words * 8); S.o_trace_off = sub.take(n_jobs * 8); S.o_trace_cap = sub.take(n_jobs * 8); S.o_trace_used = sub.take(n_jobs * 8);
+    }
     S.block_bytes = sub.end;
     return S;
 }
@@ -226,7 +244,10 @@ inline std::string retry_round(const StagePlan &S, const std::vector<int> &statu
     for (size_t j = 0; j < status.size(); ++j) {
         const int sc = status[j];
         if (sc == JOB_OK) continue;
-        if (!S.worst_case && (sc == JOB_ERR_PLANE_CAP || sc == JOB_ERR_MSA_CAP || sc == JOB_ERR_GT_CAP)) { next.jobs.push_back(S.perm[j]); continue; }
+        if (!S.worst_case && (sc == JOB_ERR_PLANE_CAP || sc == JOB_ERR_MSA_CAP || sc == JOB_ERR_GT_CAP || sc == JOB_ERR_TRACE_CAP)) {
+            next.jobs.push_back(S.perm[j]);
+            continue;
+        }
         char buf[200];
         if (sc == JOB_ERR_PLANE_CAP)
             snprintf(buf, sizeof(buf), "job %lld needs more DP-plane memory than this lane can plan (%.1f GB of planes per slot)", (long long)S.perm[j],
@@ -243,20 +264,42 @@ inline std::string retry_round(const StagePlan &S, const std::vector<int> &statu
 // job-count / byte limits of ONE device batch (larger requests are cut into chunks)
 constexpr int64_t kMaxJobsPerBatch = 1 << 15;
 constexpr int64_t kMaxBasesPerBatch = (int64_t)768 << 20;
+// a trace call's device batch: its jobs' first-round trace regions (trace_words_for_job) take at most 2 GB of its stage's block, which
+// counts against the lane's budget (lane_budget_bytes); a larger call is cut into more device batches
+constexpr int64_t kMaxTraceWordsPerBatch = (int64_t)256 << 20;
 
 // Where the device batches of `mine` (caller indices into T) end: a chunk takes jobs in order up to kMaxJobsPerBatch jobs and
-// kMaxBasesPerBatch bases, and at least one job.
-inline std::vector<size_t> chunk_ends(const JobTable &T, const std::vector<int64_t> &mine) {
+// kMaxBasesPerBatch bases, and at least one job; trace_words > 0 (a trace call): also up to that many trace words, the regions
+// planned for (grow, worst_case).
+inline std::vector<size_t> chunk_ends(const JobTable &T, const std::vector<int64_t> &mine, int64_t trace_words = 0, double grow = 1.0,
+                                      bool worst_case = false) {
     std::vector<size_t> ends;
     for (size_t at = 0; at < mine.size();) {
-        size_t end = at; int64_t bases = 0;
-        while (end < mine.size() && (int64_t)(end - at) < kMaxJobsPerBatch && (end == at || bases + T.jobs[mine[end]].sum_len <= kMaxBasesPerBatch)) {
-            bases += T.jobs[mine[end]].sum_len; ++end;
+        size_t end = at; int64_t bases = 0, words = 0;
+        auto job_words = [&](size_t k) { const TableJob &J = T.jobs[mine[k]]; return trace_words_for_job(J.n_seq, J.sum_len, J.max_len, grow, worst_case); };
+        while (end < mine.size() && (int64_t)(end - at) < kMaxJobsPerBatch &&
+               (end == at || (bases + T.jobs[mine[end]].sum_len <= kMaxBasesPerBatch && (trace_words <= 0 || words + job_words(end) <= trace_words)))) {
+            bases += T.jobs[mine[end]].sum_len;
+            if (trace_words > 0) words += job_words(end);
+            ++end;
         }
         ends.push_back(end);
         at = end;
     }
     return ends;
+}
+
+// The stages of a capacity retry `next` after a round of S: one, or for a trace stage as many as keep each one's trace regions (x4 or
+// worst case) within kMaxTraceWordsPerBatch, so that a large retry is cut like a large call instead of failing the lane's budget.
+inline std::vector<std::vector<int64_t>> retry_batches(const JobTable &T, const StagePlan &S, const RetryRound &next) {
+    if (!S.trace) return {next.jobs};
+    std::vector<std::vector<int64_t>> out;
+    size_t at = 0;
+    for (size_t end : chunk_ends(T, next.jobs, kMaxTraceWordsPerBatch, next.grow, next.worst_case)) {
+        out.emplace_back(next.jobs.begin() + at, next.jobs.begin() + end);
+        at = end;
+    }
+    return out;
 }
 
 // The table's jobs dealt over ndev devices, each device's share in caller order: one device takes everything; several take the

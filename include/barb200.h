@@ -87,6 +87,23 @@ int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, co
                           const uint8_t *seqs, const int *progressive, uint8_t **msa_out, int *msa_len,
                           int64_t *cells);
 
+/* Trace form of barb200_poa_msa_batch: the same jobs, dealt over the context's devices the same way, through trace kernels that also
+ * record every alignment the device makes. trace_out[i] = malloc'd array of n_words[i] int64 words (release with barb200_free):
+ *   n_seq, msa_len, cells                          (cells as barb200_poa_msa_batch returns them)
+ *   read_id_map[n_seq]                             the read order (guide tree): read_id_map[a] = the job's read aligned a-th
+ *   per alignment a (n_seq records, in read order):
+ *     read_id, qlen, node_n (before the alignment), n_cigar, best_score, n_rows (= node_n - 1; 0 for the first read, which
+ *     starts the graph and is not aligned; its n_cigar and best_score are 0 too)
+ *     cigar[n_cigar]                               abPOA's graph cigar words (uint64 stored as int64)
+ *     dp_beg[n_rows], dp_end[n_rows]               the adaptive band of every DP row, in topological order
+ *   the MSA, n_seq x msa_len bytes row-major, packed 8 bytes per word (the last word padded with zeros)
+ * This is the layout abPOA's own per-alignment state gives (abpoa_align_sequence_to_subgraph's graph_cigar and best score,
+ * abm->dp_beg / dp_end), so that a device run can be compared with the reference alignment by alignment. The MSAs and cells are
+ * those of barb200_poa_msa_batch. Errors as barb200_poa_msa_batch: on failure no arrays are left. For tests and diagnosis; its speed
+ * is not a goal. */
+int barb200_poa_trace_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs,
+                            const int *progressive, int64_t **trace_out, int64_t *n_words);
+
 /* Staged form of the same call for callers (and bench.py) that keep inputs resident in HBM:
  * stage = host packing + guide trees + H2D once; run = kernel(s) only, may be repeated; fetch = D2H + unpack. */
 typedef struct barb200_stage barb200_stage;

@@ -39,6 +39,16 @@ for e, job in enumerate(jobs):
     ok = msas[e].shape == tr["msa"].shape and np.array_equal(msas[e], tr["msa"]) and int(cells[e]) == tr["cells"]
     bad += not ok
 print("poa: %d jobs, %d cells, mismatches vs oracle: %d" % (len(jobs), int(cells.sum()), bad), flush=True)
+# the trace kernels, one launch per CTA class: a job whose longest read needs that class (16 T - 1 bases), two reads each
+rng1 = np.random.default_rng(12)
+for T in (32, 64, 128, 256, 640, 1024):
+    tjob = [s[:16 * T - 1] for s in family(rng1, 2, 16 * T - 1, sub=0.02, ins=0.01, dele=0.01)]
+    pn = R.cactus_params(wb=30, wf=0.002)
+    te = cb.Engine(cb.PoaParams(partialOrderAlignmentBandConstant=30, partialOrderAlignmentBandFraction=0.002, threads_per_block=T))
+    d = cb.first_trace_difference(te.poa_msa_trace_batch([tjob])[0], R.oracle_poa_msa_trace(tjob, pn))
+    te.close()
+    bad += d is not None
+    print("trace t%d: identical to the oracle: %s" % (T, d is None), flush=True)
 seqs = [bytes(np.frombuffer(b"ACGT", np.uint8)[np.random.default_rng(5).integers(0, 4, 900)]) for _ in range(1)]
 base = seqs[0]
 fam = [base, base[:400] + base[420:], base[:100] + b"ACGT" + base[100:], base[5:880]]
