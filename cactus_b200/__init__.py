@@ -5,7 +5,9 @@ Python mirror of the reference's POA entry points (bar/inc/poaBarAligner.h) on t
 :class:`Engine` without a CUDA device (or without the built library) raises -- there is no CPU fallback.
 """
 from .api import (Engine, Msa, BarB200Error, PoaParams, PairwiseAlignmentParameters, MumParams, load_library, library_path,
-                  msa_to_base, msa_to_byte, parse_trace, first_trace_difference, pecan_band, pecan_split_points)
+                  msa_to_base, msa_to_byte, parse_trace, first_trace_difference, parse_end_trace, first_end_trace_difference,
+                  pecan_band, pecan_split_points)
 
 __all__ = ["Engine", "Msa", "BarB200Error", "PoaParams", "PairwiseAlignmentParameters", "MumParams", "load_library", "library_path",
-           "msa_to_base", "msa_to_byte", "parse_trace", "first_trace_difference", "pecan_band", "pecan_split_points"]
+           "msa_to_base", "msa_to_byte", "parse_trace", "first_trace_difference", "parse_end_trace",
+           "first_end_trace_difference", "pecan_band", "pecan_split_points"]

@@ -76,6 +76,8 @@ def load_library():
     lib.barb200_poa_msa_batch.restype = ci
     lib.barb200_poa_trace_batch.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp]
     lib.barb200_poa_trace_batch.restype = ci
+    lib.barb200_trace_ends.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp, i64, i64, C.c_double, vp, vp]
+    lib.barb200_trace_ends.restype = ci
     lib.barb200_stage_create.argtypes = [vp, i64, vp, vp, vp, vp, C.POINTER(vp)]
     lib.barb200_stage_create.restype = ci
     lib.barb200_stage_run.argtypes = [vp, C.POINTER(C.c_float)]
@@ -210,6 +212,70 @@ def first_trace_difference(got, want):
                 return (a, k, int(bad[0]))
     if len(got["alns"]) != len(want["alns"]):
         return (None, "alns", None)
+    return None
+
+
+def parse_end_trace(words):
+    """One end's trace words (barb200_trace_ends, layout in include/barb200.h) as a dict: seq_no, windows = one dict per window in
+    chain order (index, offsets, lens, empty (int64 per row), progressive, trace = the window's job as :func:`parse_trace` gives
+    it, trimmed_lens, column_no) and msa = the end's final MSA (uint8 [seq_no, column_no])."""
+    w = np.asarray(words, np.int64)
+    K, n_win = int(w[0]), int(w[1])
+    pos = 2
+    windows = []
+    for _ in range(n_win):
+        index = int(w[pos])
+        pos += 1
+        offsets, lens, empty = (w[pos + i * K:pos + (i + 1) * K].copy() for i in range(3))
+        pos += 3 * K
+        progressive, n_trace = int(w[pos]), int(w[pos + 1])
+        pos += 2
+        trace = parse_trace(w[pos:pos + n_trace], K)
+        pos += n_trace
+        trimmed = w[pos:pos + K].copy()
+        column_no = int(w[pos + K])
+        pos += K + 1
+        windows.append(dict(index=index, offsets=offsets, lens=lens, empty=empty, progressive=progressive, trace=trace,
+                            trimmed_lens=trimmed, column_no=column_no))
+    if int(w[pos]) != K:
+        raise ValueError("end trace: MSA of %d rows, expected %d" % (int(w[pos]), K))
+    cols = int(w[pos + 1])
+    pos += 2
+    msa = w[pos:].view(np.uint8)[: K * cols].reshape(K, cols).copy()
+    if len(w) != pos + (K * cols + 7) // 8:
+        raise ValueError("end trace: %d words, layout gives %d" % (len(w), pos + (K * cols + 7) // 8))
+    return dict(seq_no=K, windows=windows, msa=msa)
+
+
+def first_end_trace_difference(got, want):
+    """Where two traces of one end (dicts of :func:`parse_end_trace`) first differ: None, or (window, field, index).
+    Windows are compared in chain order, each by its input (offsets, lens, empty: index = the first differing row; progressive) and
+    then its job's trace (field "trace", index = the (alignment, field, index) of :func:`first_trace_difference`). A window's
+    trimmed_lens and column_no are compared only after every window's input and trace, since trimming window n also depends on
+    window n+1. Then the window count ("n_windows"), and last the end's final MSA ("msa", window None)."""
+    if got["seq_no"] != want["seq_no"]:
+        return (None, "seq_no", None)
+    gw, ww = got["windows"], want["windows"]
+    for k, (x, y) in enumerate(zip(gw, ww)):
+        for f in ("offsets", "lens", "empty"):
+            bad = np.flatnonzero(np.asarray(x[f]) != np.asarray(y[f]))
+            if len(bad):
+                return (k, f, int(bad[0]))
+        if x["progressive"] != y["progressive"]:
+            return (k, "progressive", None)
+        d = first_trace_difference(x["trace"], y["trace"])
+        if d is not None:
+            return (k, "trace", d)
+    if len(gw) != len(ww):
+        return (min(len(gw), len(ww)), "n_windows", "count %d vs %d" % (len(gw), len(ww)))
+    for k, (x, y) in enumerate(zip(gw, ww)):
+        bad = np.flatnonzero(np.asarray(x["trimmed_lens"]) != np.asarray(y["trimmed_lens"]))
+        if len(bad):
+            return (k, "trimmed_lens", int(bad[0]))
+        if x["column_no"] != y["column_no"]:
+            return (k, "column_no", None)
+    if got["msa"].shape != want["msa"].shape or not np.array_equal(got["msa"], want["msa"]):
+        return (None, "msa", None)
     return None
 
 
@@ -636,6 +702,36 @@ class Engine:
         out = [self._wrap(ms[i]) for i in range(n)]
         self.lib.barb200_free(C.cast(ms, C.c_void_p))
         return out
+
+    def trace_ends(self, ends, right_end_indexes=None, right_end_row_indexes=None, overlaps=None, window_size=10000,
+                   max_prog_rows=5000, max_prog_length_diff=1.0):
+        """barb200_trace_ends: every sliding window of every end, with the arguments of make_consistent_partial_order_alignments
+        (without the index lists the ends are independent). One dict of :func:`parse_end_trace` per end: each window's input slice,
+        its POA job's per-alignment trace and its trimmed lengths, and the end's final MSA."""
+        t = _StrTable(ends)
+        n = len(ends)
+        keep = []
+
+        def table(rows):
+            if rows is None:
+                return None
+            arr = (C.c_void_p * max(n, 1))()
+            for i, r in enumerate(rows):
+                a = (C.c_int64 * max(len(r), 1))(*[int(v) for v in r])
+                keep.append(a)
+                arr[i] = C.cast(a, C.c_void_p)
+            return arr
+        outs = (C.c_void_p * max(n, 1))()
+        nw = np.zeros(max(n, 1), np.int64)
+        self._check(self.lib.barb200_trace_ends(self.ctx, n, t.seq_no, t.strs, t.lens, table(right_end_indexes),
+                                                table(right_end_row_indexes), table(overlaps), window_size, max_prog_rows,
+                                                max_prog_length_diff, outs, nw.ctypes.data))
+        res = []
+        for i in range(n):
+            w = np.ctypeslib.as_array(C.cast(outs[i], C.POINTER(C.c_int64)), shape=(int(nw[i]),)).copy()
+            self.lib.barb200_free(outs[i])
+            res.append(parse_end_trace(w))
+        return res
 
     # ---- the end queue, asynchronously (barb200_flower_submit / barb200_flower_wait) ---------------------------------
     def flower_submit(self, end_strings, right_end_indexes=None, right_end_row_indexes=None, overlaps=None,

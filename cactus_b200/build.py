@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbarb200.so")
-SOURCES = ["poa_kernel.cu", "poa_trace_kernel.cu", "guide_tree.cu", "barb200.cu", "host_bar.cpp", "pecan.cu", "pecan_plan.cpp", "mum_anchor.cu"]
+SOURCES = ["poa_kernel.cu", "poa_trace_kernel.cu", "guide_tree.cu", "barb200.cu", "host_bar.cpp", "host_end_trace.cpp","pecan.cu", "pecan_plan.cpp", "mum_anchor.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fopenmp,-O3,-Wall,-Wno-unused-function", "-Xptxas", "-v"]

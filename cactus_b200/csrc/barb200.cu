@@ -874,4 +874,24 @@ int run_jobs_on_lane(barb200_ctx *ctx, int lane, const std::vector<HostJob> &job
     for (int64_t j = 0; j < n; ++j) { results[j].msa_len = ml[j]; results[j].cells = cells[j]; }
     return BARB200_OK;
 }
+
+// host jobs as one barb200_poa_trace_batch call (host_end_trace.cpp's rounds)
+int run_trace_jobs(barb200_ctx *ctx, const std::vector<HostJob> &jobs, std::vector<std::vector<int64_t>> &words) {
+    const int64_t n = (int64_t)jobs.size();
+    words.assign(n, std::vector<int64_t>());
+    if (n == 0) return BARB200_OK;
+    std::vector<int> n_seq(n), prog(n), lens; std::vector<uint8_t> seqs;
+    for (int64_t j = 0; j < n; ++j) {
+        const HostJob &J = jobs[j];
+        n_seq[j] = J.n_seq; prog[j] = J.progressive;
+        int64_t sum = 0;
+        for (int i = 0; i < J.n_seq; ++i) { lens.push_back(J.lens[i]); sum += J.lens[i]; }
+        seqs.insert(seqs.end(), J.seqs, J.seqs + sum);
+    }
+    std::vector<int64_t *> out(n, nullptr); std::vector<int64_t> nw(n, 0);
+    const int rc = barb200_poa_trace_batch(ctx, n, n_seq.data(), lens.data(), seqs.data(), prog.data(), out.data(), nw.data());
+    if (rc) return rc;
+    for (int64_t j = 0; j < n; ++j) { words[j].assign(out[j], out[j] + nw[j]); free(out[j]); }
+    return BARB200_OK;
+}
 }  // namespace barb200

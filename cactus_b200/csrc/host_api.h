@@ -47,6 +47,9 @@ struct JobResult {
 // barb200.cu: one device batch of host jobs on device lane `lane` (0 .. total_lanes-1; bucketed by CTA class, capacity misses
 // retried with larger slots). Returns a BARB200_* code; the message is get_error(ctx).
 int run_jobs_on_lane(barb200_ctx *ctx, int lane, const std::vector<HostJob> &jobs, std::vector<JobResult> &results);
+// barb200.cu: host jobs as trace jobs, through barb200_poa_trace_batch (its job checks, deal over the context's devices, batches and
+// capacity retries); words[j] = job j's trace in that call's layout (include/barb200.h). barb200_trace_ends' device layer.
+int run_trace_jobs(barb200_ctx *ctx, const std::vector<HostJob> &jobs, std::vector<std::vector<int64_t>> &words);
 int total_lanes(barb200_ctx *ctx);
 void **dispatcher_slot(barb200_ctx *ctx);         // where host_bar.cpp keeps the context's end queue
 void mark_lanes_shared(barb200_ctx *ctx);

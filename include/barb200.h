@@ -104,6 +104,32 @@ int barb200_poa_msa_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, co
 int barb200_poa_trace_batch(barb200_ctx *ctx, int64_t n_jobs, const int *n_seq, const int *seq_lens, const uint8_t *seqs,
                             const int *progressive, int64_t **trace_out, int64_t *n_words);
 
+/* Trace form of barb200_make_consistent_partial_order_alignments (arguments as barb200_flower_submit; right_end_indexes == NULL:
+ * independent ends): every sliding window of every end, window by window. Window n+1 of an end is cut at offsets that window n's
+ * trimmed MSA decides, so a window cannot be checked on its own; this call records the whole chain. trace_out[e] = malloc'd array
+ * of n_words[e] int64 words per end (release each with barb200_free), K = the end's string count:
+ *   K, n_windows                                   (no windows for a single string or an end without bases)
+ *   per window, in chain order:
+ *     window index (0, 1, ...)
+ *     offset[K]                                    where each row's slice starts in its string
+ *     len[K]                                       the slice lengths the POA job gets (1 for a row given the N stand-in)
+ *     empty[K]                                     1: the row ran out of bases and got the N stand-in (poaBarAligner.c:551-562)
+ *     progressive                                  the job's progressive flag (:567-571)
+ *     n_trace, trace[n_trace]                      the window's POA job, word for word in barb200_poa_trace_batch's layout
+ *     trimmed_len[K], column_no                    the window's row lengths and columns after trimming against both neighbours,
+ *                                                  as the stitch uses them
+ *   K, column_no, the end's MSA                    stitched and trimmed across ends: barb200_make_consistent_partial_order_
+ *                                                  alignments' MSA, K x column_no bytes row-major, packed 8 bytes per word
+ * The windows run through the same window, trim and stitch steps as the end queue, in synchronous rounds (the next window of every
+ * unfinished end in one trace call), not through the queue's batches: a window's result depends on its job alone. Not covered:
+ * the production kernels' node order (traces number rows in abPOA's BFS order, as barb200_poa_trace_batch does) and the queue's
+ * batching, which the final MSAs check. Errors as barb200_make_consistent_partial_order_alignments, with its messages; the return
+ * is a BARB200_* code and on failure no arrays are left. For diagnosis; its speed is not a goal. */
+int barb200_trace_ends(barb200_ctx *ctx, int64_t end_no, const int64_t *end_lengths, char ***end_strings,
+                       int **end_string_lengths, int64_t **right_end_indexes, int64_t **right_end_row_indexes, int64_t **overlaps,
+                       int64_t window_size, int64_t max_prog_rows, double max_prog_length_diff, int64_t **trace_out,
+                       int64_t *n_words);
+
 /* Staged form of the same call for callers (and bench.py) that keep inputs resident in HBM:
  * stage = host packing + guide trees + H2D once; run = kernel(s) only, may be repeated; fetch = D2H + unpack. */
 typedef struct barb200_stage barb200_stage;
